@@ -5,6 +5,7 @@ Default workload (BASELINE configs[1], `--config 2`): celeba_hq.yml denoiser (ra
 pooling), sigma_y=0, T_sampling=100, eta=0.85, 16 images per GPU.  A "step" = one full sampling of the per-GPU batch.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config 2|3|4|5a|5b] [--precision fp32|fp16]
+                    [--dump-outputs DIR]
 
 `value`  : the loop with x_T / y resident in HBM; the per-pair Gaussian draws ARE inside the timed region (drawn chunk by chunk on a
            side stream by ddnm_b200.sampler, like the reference's one randn_like per step).
@@ -12,8 +13,9 @@ pooling), sigma_y=0, T_sampling=100, eta=0.85, 16 images per GPU.  A "step" = on
 N>1 is launched by torchrun (one rank per GPU): rows shard over ranks, no traffic inside the loop, one all-gather of the restored
 images per step (weak scaling); an untimed sharded-vs-unsharded check runs first (`shard_check`).
 `--impl reference` times the UNMODIFIED reference (oracle/_ref, see oracle/make_ref.py) on the host cores on a bounded sample.
-The other BASELINE configs (`--config 3|4|5a|5b`) and the fp16 fast mode print the same line for their workload; their results are
-kept under profiles/ (the driver's N=1 line stays configs[1]).
+The other BASELINE configs (`--config 3|4|5a|5b`) and the fp16 fast mode print the same line for their workload.
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (x_0 and x0_pred of the batch) as float32 .npy files
+under DIR, so that two builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -52,7 +54,8 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return dict(hbm=p["hbm_gbs"], tf_burst=p["bf16_tflops"], tf_sust=p["bf16_tflops_sustained"], src="measured (MEASURED_PEAKS.json)")
     except Exception:
-        return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback (B200_PROFILING.md)")
+        # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16/BF16 — never reached, an upper bound only
+        return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet (not measured)")
 
 
 def sampler_cfg(c):
@@ -62,7 +65,7 @@ def sampler_cfg(c):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled every 200 ms during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled every 200 ms during the timed region (read-only queries)."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, gpu_index):
@@ -106,9 +109,8 @@ class ClockSampler:
         return out
 
 
-# torch's CPU conv path collapses when oversubscribed: measured on the B200 host (128 hw threads) one image-forward takes 1.07 s at
-# 8 threads, 1.20 s at 16, 1.25 s at 32, 1.92 s at 64 and 51.5 s at 128 (profiles/r01_cpu_threads.txt), so the CPU arms run at the
-# thread count where the reference is fastest
+# torch's CPU conv path collapses when oversubscribed (one image-forward of the reference gets slower beyond ~16 threads on a
+# many-core host), so the CPU arms run at no more than 16 threads
 def cpu_threads():
     return min(os.cpu_count() or 1, 16)
 
@@ -216,6 +218,23 @@ def build_workload(c, dev, precision):
     return model, op, c["sigma_y"] > 0
 
 
+DUMP_BUDGET = 64_000_000 - 4096   # bytes written by --dump-outputs, .npy headers included
+
+
+def dump_outputs(d, arrays):
+    """Each array as DIR/<name>.npy in float32.  Beyond an equal share of DUMP_BUDGET an array is replaced by a fixed, seeded sample of
+    its flattened elements (the same positions on every run of the same shape)."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    share = DUMP_BUDGET // len(arrays) // 4
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.size > share:
+            idx = np.sort(np.random.default_rng(1234).choice(a.size, share, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(d, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def main():
     # exactly ONE line on stdout: libraries (NCCL prints its version banner) write to fd 1, so park the real stdout and
     # point fd 1 at stderr until the JSON line is ready
@@ -235,9 +254,11 @@ def main():
     ap.add_argument("--precision", default="fp32", choices=["fp32", "fp16"],
                     help="fp32 = fp32-grade 3x fp16 products (parity mode); fp16 = 1 product per MAC, the analogue of use_fp16 (NOT parity grade)")
     ap.add_argument("--batch", type=int, default=0, help="images per GPU (default: the config's)")
-    ap.add_argument("--e2e-steps", type=int, default=0, help="timed steps of the end-to-end leg (default max(5, steps))")
+    ap.add_argument("--e2e-steps", type=int, default=0, help="timed steps of the end-to-end leg (default: --steps)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--profile-steps", type=int, default=0, help="(ncu runs) skip the e2e / baseline legs")
+    ap.add_argument("--profile-steps", type=int, default=0, help="(profiler runs) skip the e2e / baseline legs")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's outputs (x0, x0_pred) as float32 .npy files under DIR (at most 64 MB in all)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args, emit)
@@ -304,13 +325,17 @@ def main():
                            note="parallel.sharded_sample over the global batch vs each rank recomputing the next rank's rows; bit-identical expected")
         del xs_g, tape, ys_g, full0, mine
 
+    last = {}
+
     def step_device():
         # hot path with x_T / y resident in HBM, draws included (+ the single end-of-run all-gather when N > 1)
         x0, x0p = local_fn(x_T_dev, y_dev)
+        last["out"] = (x0, x0p)
         if world == 1:
             return x0, x0p
         outs = [torch.empty_like(x0) for _ in range(world)]
         dist.all_gather(outs, x0)
+        last["out"] = (torch.cat(outs), x0p)
         return outs, x0p
 
     def step_e2e():
@@ -338,7 +363,7 @@ def main():
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return ms.item()
 
-    if args.profile_steps:      # ncu launch list: just run the hot path
+    if args.profile_steps:      # profiler launch list: just run the hot path
         for _ in range(args.profile_steps):
             step_device()
         torch.cuda.synchronize()
@@ -349,7 +374,15 @@ def main():
     clocks.start()
     ms_total = timed(step_device, args.steps, args.warmup)
     clk = clocks.stop()
-    e2e_steps = args.e2e_steps or max(5, args.steps)
+    if args.dump_outputs:
+        x0_all, x0p = last["out"]
+        if world > 1:   # x0_pred of every rank (outside the timed region: the timed step gathers x0 only)
+            parts = [torch.empty_like(x0p) for _ in range(world)]
+            dist.all_gather(parts, x0p)
+            x0p = torch.cat(parts)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, dict(x0=x0_all, x0_pred=x0p))
+    e2e_steps = args.e2e_steps or args.steps
     ms_e2e = timed(step_e2e, e2e_steps, 2)
     ms_step = ms_total / args.steps
     value = Bg * 1e3 / ms_step
@@ -358,34 +391,24 @@ def main():
     if rank == 0:
         info = model.info(B)
         pk = peaks()
-        # roofline of the dominant kernel family (the tcgen05 convolution): per-launch CUDA-event timing of one eager forward
+        # roofline of the dominant kernel family (the wgmma convolution): per-launch CUDA-event timing of one eager forward
         xt = torch.randn(B, 3, RES, RES, device=dev)
         # three eager passes, per launch the fastest: in the regions of short launches the elapsed time between two events measures the
-        # host's issue rate rather than the kernel (profiles/r02_attn_anomaly.md), and that jitter is one-sided
+        # host's issue rate rather than the kernel, and that jitter is one-sided
         tt = torch.full((B,), 500.0, device=dev)
         prof = model.profile(xt, tt)
         for _ in range(2):
             for a, b in zip(prof, model.profile(xt, tt)):
                 a["ms"] = min(a["ms"], b["ms"])
-        tc = [p for p in prof if p["kind"] in ("tc", "tcgn")]
+        tc = [p for p in prof if p["kind"] == "tc"]
         tc_ms, tc_fl = sum(p["ms"] for p in tc), sum(p["flops"] for p in tc)
         all_ms = sum(p["ms"] for p in prof)
         ach = tc_fl / tc_ms / 1e9 if tc_ms > 0 else 0.0
         fwd_launches = sum(4 if p["kind"] == "temb" else (0 if p["kind"] == "memset" else 1) for p in prof)
-        traffic = None
-        for src in ("r02_conv_traffic.json", "r01_conv_tc_traffic.json"):
-            try:   # STATIC: one `ncu --set full` capture of the top launch kept under profiles/ (not re-measured in this run)
-                tj = json.load(open(os.path.join(ROOT, "profiles", src)))["top_launch"]
-                traffic = dict(bytes=tj["traffic_bytes"], algorithmic_bytes=tj["algorithmic_bytes"], launch=tj["name"],
-                               tensor_pipe_active_pct=tj["tensor_pipe_active_pct"],
-                               source=f"static: profiles/{src} (ncu --set full capture of this launch, not re-measured by this run)")
-                break
-            except Exception:
-                pass
         terms = 3 if args.precision == "fp32" else 1
-        roof = dict(bound="tensor", kernel="conv_tc_kernel / conv_gn_tc_kernel (tcgen05 implicit GEMM, TMA-staged, TMEM accumulators)", achieved=ach,
+        roof = dict(bound="tensor", kernel="conv_tc_kernel (wgmma implicit GEMM, TMA-staged, register accumulators)", achieved=ach,
                     peak=pk["tf_sust"], unit="TFLOP/s", frac=ach / pk["tf_sust"], hw_mma_factor=terms, frac_hw=terms * ach / pk["tf_sust"],
-                    peak_source=pk["src"] + ", sustained bf16 cuBLAS", traffic=traffic,
+                    peak_source=pk["src"],
                     launches_per_forward=len(tc), avg_launch_ms=tc_ms / max(1, len(tc)), share_of_forward=tc_ms / all_ms,
                     note=f"achieved = algorithmic conv/GEMM FLOPs (2*M*N*K once) / summed per-launch CUDA-event time; each algorithmic MAC costs {terms} fp16 MMA(s)"
                          + (" (hi*hi+hi*lo+lo*hi) for fp32-grade products, so frac_hw = 3*frac is the tensor-pipe utilisation and 1/3 the ceiling of frac" if terms == 3 else ""))
@@ -394,7 +417,8 @@ def main():
                     config=dict(workload=c["workload"], baseline_config=args.config, precision=args.precision, global_batch=Bg,
                                 parallelism=f"rows sharded over {world} GPU(s), 1 all-gather at the end",
                                 noise="per-pair Gaussian draws inside the timed region (side stream, bounded double buffer)",
-                                l2="working set per UNet forward (GiBs of activations) exceeds the 126 MB L2; no flush needed",
+                                l2="working set per UNet forward (GiBs of activations) exceeds the 50 MB L2; no flush needed",
+                                gpu=torch.cuda.get_device_name(dev),
                                 unet_ms_per_forward=all_ms, unet_evals_per_image=evals, time_pairs=n_pairs,
                                 unet_flops_per_image_forward=info["flops_per_forward"] / B, workspace_bytes=info["workspace_bytes"]),
                     clocks=clk, roofline=roof,

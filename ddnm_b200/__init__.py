@@ -1,4 +1,4 @@
-"""ddnm_b200 — B200-native DDNM sampling engine (hand-written sm_100a CUDA behind a C ABI).
+"""ddnm_b200 — H100-native DDNM sampling engine (hand-written sm_90a CUDA behind a C ABI).
 
 Public surface mirrors the reference's hot path (wyhuai/DDNM):
   ddnm_b200.model.Model                      <- guided_diffusion/models.py::Model  (``et = model(xt, t)``)

@@ -1,4 +1,4 @@
-"""Build libddnm_b200.so (sm_100a only) with nvcc; sources in ddnm_b200/csrc, objects in build/, the shared
+"""Build libddnm_b200.so (sm_90a only) with nvcc; sources in ddnm_b200/csrc, objects in build/, the shared
 library lands IN-TREE next to this file so it travels with the repo snapshot to the GPU box."""
 import concurrent.futures as cf
 import os
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(ROOT, "build", "obj")
 LIB = os.path.join(HERE, "libddnm_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
          "-DDDNM_BUILD"]
 
 
@@ -27,6 +27,7 @@ def build(force=False, verbose=False):
     srcs = sorted(f for f in os.listdir(CSRC) if f.endswith(".cu"))
     hdrs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     hdrs.append(os.path.join(ROOT, "include", "ddnm_b200.h"))
+    hdrs.append(os.path.abspath(__file__))   # FLAGS (the target architecture) live here: objects older than them are rebuilt
     jobs = []
     for s in srcs:
         src, obj = os.path.join(CSRC, s), os.path.join(OBJ, s[:-3] + ".o")
@@ -46,8 +47,8 @@ def build(force=False, verbose=False):
     with cf.ThreadPoolExecutor(max_workers=min(8, max(1, len(jobs)))) as ex:
         list(ex.map(cc, jobs))
     objs = [os.path.join(OBJ, s[:-3] + ".o") for s in srcs]
-    if jobs or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    if jobs or _newer(os.path.abspath(__file__), LIB, []):
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -368,8 +368,8 @@ int ddnm_groupnorm(const float* x, int N, int H, int W, int C, int groups, const
   DDNM_API_END
 }
 
-// out = conv3x3(silu?(groupnorm(x))) [+ conv1x1(side_x)] + bias [+ residual] through the FUSED kernel (tc_gn_conv.cu); gamma == NULL
-// skips the normalisation.  iters > 0: also time `iters` launches (ms_per_iter may be NULL otherwise).
+// out = conv3x3(silu?(groupnorm(x))) [+ conv1x1(side_x)] + bias [+ residual] through the fused GN form of the convolution kernel;
+// gamma == NULL skips the normalisation.  iters > 0: also time `iters` launches (ms_per_iter may be NULL otherwise).
 int ddnm_conv_gn_tc(const float* x, int N, int H, int W, int Cin, int groups, const float* gamma, const float* beta, float eps, int silu,
                     const float* w, const float* bias, int Cout, const float* side_x, int CinSide, const float* side_w,
                     const float* residual, float* out, int iters, float* ms_per_iter, void* stream) {
@@ -392,15 +392,15 @@ int ddnm_conv_gn_tc(const float* x, int N, int H, int W, int Cin, int groups, co
   GnAffine gn;
   gn.gamma = gamma; gn.beta = beta; gn.eps = eps; gn.groups = groups; gn.silu = silu != 0;
   View ov = mkview(out, N, H, W, Cout);
-  TcGnLaunch L = tc_make_gn_launch(xv, gn, side_x ? &sv : nullptr, wh, wl, Cout, ov, bias, 0, residual, Cout, sm_count());
-  tc_gn_run(L, s);
+  TcLaunch L = tc_make_gn_launch(xv, gn, side_x ? &sv : nullptr, wh, wl, Cout, ov, bias, 0, residual, Cout, sm_count());
+  tc_run(L, s);
   if (iters > 0 && ms_per_iter) {
     cudaEvent_t e0, e1;
     CUDA_CHECK(cudaEventCreate(&e0));
     CUDA_CHECK(cudaEventCreate(&e1));
-    for (int i = 0; i < 2; ++i) tc_gn_run(L, s);
+    for (int i = 0; i < 2; ++i) tc_run(L, s);
     CUDA_CHECK(cudaEventRecord(e0, s));
-    for (int i = 0; i < iters; ++i) tc_gn_run(L, s);
+    for (int i = 0; i < iters; ++i) tc_run(L, s);
     CUDA_CHECK(cudaEventRecord(e1, s));
     CUDA_CHECK(cudaEventSynchronize(e1));
     float ms = 0;
@@ -412,27 +412,16 @@ int ddnm_conv_gn_tc(const float* x, int N, int H, int W, int Cin, int groups, co
   CUDA_CHECK(cudaStreamSynchronize(s));
   DDNM_API_END
 }
-int ddnm_tc_debug_gn_counters(long long* dev_buf) {
-  DDNM_API_BEGIN
-  tc_debug_gn_counters(dev_buf);
-  DDNM_API_END
-}
-int ddnm_tc_debug_gn_pf_dist(int d) {
-  DDNM_API_BEGIN
-  tc_debug_gn_pf_dist(d);
-  DDNM_API_END
-}
-int ddnm_tc_debug_gn_desc_mode(int mode) {
-  DDNM_API_BEGIN
-  tc_debug_gn_desc_mode(mode);
-  DDNM_API_END
-}
 int ddnm_tc_debug_gn_fused(int on) {
   DDNM_API_BEGIN
   tc_debug_gn_fused(on);
   DDNM_API_END
 }
-
+int ddnm_tc_debug_deal(int mode) {
+  DDNM_API_BEGIN
+  tc_debug_deal(mode);
+  DDNM_API_END
+}
 int ddnm_tc_debug_pair_mode(int mode) {
   DDNM_API_BEGIN
   tc_debug_pair_mode(mode);
@@ -448,25 +437,9 @@ int ddnm_tc_debug_pair_dual(int on) {
   tc_debug_pair_dual(on);
   DDNM_API_END
 }
-int ddnm_tc_debug_halo(int on) {
-  DDNM_API_BEGIN
-  tc_debug_halo(on);
-  DDNM_API_END
-}
-int ddnm_tc_debug_deal(int mode) {
-  DDNM_API_BEGIN
-  tc_debug_deal(mode);
-  DDNM_API_END
-}
 int ddnm_tc_debug_force_bn(int bn) {
   DDNM_API_BEGIN
   tc_debug_force_bn(bn);
   DDNM_API_END
 }
-int ddnm_tc_debug_override(unsigned desc_hi, unsigned idesc_xor) {
-  DDNM_API_BEGIN
-  tc_debug_override(desc_hi, idesc_xor);
-  DDNM_API_END
-}
-
 }  // extern "C"

@@ -34,7 +34,7 @@ UNetEngine::UNetEngine(int batch, int in_channels, int out_ch, int resolution, i
   CUDA_CHECK(cudaGetDevice(&dev));
   cudaDeviceProp prop;
   CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-  DDNM_CHECK(prop.major == 10, "ddnm_b200 kernels are built for sm_100a (B200) only");
+  DDNM_CHECK(prop.major == 9 && prop.minor == 0, "ddnm_b200 kernels are built for sm_90a (H100) only");
   num_sms_ = prop.multiProcessorCount;
 }
 
@@ -162,7 +162,7 @@ void UNetEngine::emit_tc(const std::string& name, const SplitView& a, int mode, 
   // 2 or 4 CTAs per tile, each over its own k-block range into its own partial buffer, then one small deterministic reduce
   const int tiles = L.p.tiles_x * L.p.tiles_y * L.p.tiles_n * L.p.n_tiles, kblocks = L.p.kb0 + L.p.kb1;
   static const bool split_on = std::getenv("DDNM_SPLITK") == nullptr || std::atoi(std::getenv("DDNM_SPLITK")) != 0;
-  if (split_on && !L.pair && !L.halo && res_mode == 0 && 2 * tiles <= num_sms_ && kblocks >= 32) {
+  if (split_on && !L.pair && res_mode == 0 && 2 * tiles <= num_sms_ && kblocks >= 32) {
     const int S = 4 * tiles <= num_sms_ ? 4 : 2;
     const long long stride = out.pixels() * Cout;
     float* part = (float*)arena_.alloc((size_t)S * stride * sizeof(float));
@@ -195,11 +195,11 @@ void UNetEngine::emit_tcgn(const std::string& name, const View& x, const std::st
   gn.silu = true;
   gn.ss = ss;
   gn.ss_ld = ss_ld;
-  TcGnLaunch L = tc_make_gn_launch(x, gn, side, w.hi, w.lo, Cout, out, chanadd, ca_ld, residual, ldr, num_sms_);
+  TcLaunch L = tc_make_gn_launch(x, gn, side, w.hi, w.lo, Cout, out, chanadd, ca_ld, residual, ldr, num_sms_);
   // algorithmic HBM bytes: the fp32 activation(s) in, the weights, the fp32 output (+ residual) — no fp16 planes
   const double bytes = (double)x.pixels() * x.C * 4 + (side ? (double)side->pixels() * side->C * 4 : 0) + (double)Cout * w.ktot * 4 +
                        (double)out.pixels() * Cout * 4 * (residual ? 2 : 1);
-  add_op(name, "tcgn", L.flops, bytes, [L](cudaStream_t s) { tc_gn_run(L, s); });
+  add_op(name, "tc", L.flops, bytes, [L](cudaStream_t s) { tc_run(L, s); });
 }
 
 // scratch every program needs; split planes are shared by all convolutions of a forward (stream order serialises them)

@@ -104,8 +104,8 @@ class UNetEngine {
                      const float* ss = nullptr, int ss_ld = 0, SplitView* raw = nullptr);
   void emit_tc(const std::string& name, const SplitView& a, int mode, const SplitView* side, const TcWeights& w, int Cout,
                const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int res_mode = 0);
-  // fused form of emit_gn_split + emit_tc for 3x3 convolutions on rows >= 128 pixels wide (tc_gn_conv.cu): x is normalised (norm =
-  // parameter prefix), activated, split and convolved in one kernel; side = raw fp32 input of a 1x1 shortcut (extra K blocks)
+  // fused form of emit_gn_split + emit_tc for 3x3 convolutions on rows >= 128 pixels wide (the GN form of conv_tc_kernel): x is
+  // normalised (norm = parameter prefix), activated, split and convolved in one kernel; side = raw fp32 input of a 1x1 shortcut
   bool fused_ok(const View& x, const View* side, int Cout, const View& out) const;
   void emit_tcgn(const std::string& name, const View& x, const std::string& norm, const float* ss, int ss_ld, const View* side,
                  const TcWeights& w, int Cout, const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr);
@@ -127,7 +127,7 @@ class UNetEngine {
 
   int B_, in_ch_, out_ch_, R_, groups_;
   float eps_;
-  int num_sms_ = 148;
+  int num_sms_ = 132;
   bool finalized_ = false, use_graph_ = true;
   int terms_ = 3;
   Arena arena_;

@@ -20,11 +20,6 @@ __device__ __forceinline__ float swishf(float x) { return x / (1.0f + expf(-x));
 // x * sigmoid(x) on the special-function unit: 2^(-x log2 e) by ex2.approx, the quotient by rcp.approx (relative error ~2e-7, two
 // orders below the fp16 split that follows it).  The GroupNorm pass is within ~1.4x of being issue-bound with the library expf and
 // the IEEE division (~20 instructions per element); this form is 5.
-__device__ __forceinline__ float swishf_fast(float x) {
-  float e;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * -1.4426950408889634f));
-  return __fdividef(x, 1.0f + e);
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // Per-channel sums for GroupNorm (torch.nn.GroupNorm(32, C): models.py:32-33 / nn.py:17-19) of a tensor that was NOT
@@ -258,7 +253,10 @@ static void gn_apply_launch(const View& x, int groups, bool normalise, const flo
   const int C8 = x.C / 8;
   const int rows = std::max(1, 256 / C8);
   const int threads = C8 * rows;
-  long long want = cdivll((long long)HW * x.N, 148 * 8);
+  int dev = 0, sms = 0;
+  CUDA_CHECK(cudaGetDevice(&dev));
+  CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  long long want = cdivll((long long)HW * x.N, (long long)sms * 8);   // ~8 CTAs per SM
   int ppc = (int)std::max<long long>(rows, cdivll(want, rows) * rows);
   dim3 grid(cdiv(HW, ppc), x.N);
   const size_t smem = (size_t)x.C * 24;   // 2 doubles + 2 floats per channel (<= 48 KiB at MAX_C)
@@ -587,7 +585,9 @@ void splitk_reduce(const float* part, int S, long long stride, const View& out, 
                    int ldr, cudaStream_t st) {
   DDNM_CHECK(out.C % 4 == 0 && out.ld % 4 == 0 && S >= 2, "split-K reduce: unsupported shape");
   const int HW = out.H * out.W;
-  const int ppc = std::max(1, (int)cdivll((long long)HW * out.N, 296));
+  // 16 CTAs per image: the pixel ranges (and so an image's fp32 partial GroupNorm sums) do not depend on the batch it runs in,
+  // which keeps a row's result bit-identical between engines of different batch sizes
+  const int ppc = std::max(1, cdiv(HW, 16));
   dim3 grid(cdiv(HW, ppc), out.N);
   launch_pdl(splitk_reduce_kernel, grid, dim3(std::min(256, out.C / 4)), 0, st, 1, part, S, stride, HW, out.C, out.p, out.ld, chanadd, ca_ld, residual,
              ldr, out.st, out.st_ld, ppc);

@@ -1,107 +1,109 @@
-// tcgen05 implicit-GEMM convolution for sm_100a.
+// wgmma implicit-GEMM convolution for sm_90a.
 //
 //   out[pixel, co] = alpha * sum_k A[pixel, k] * Wt[co, k] + chanadd[image, co] + residual[pixel, co]
 //
 // A is never materialised: for k-block (tap, 64-channel slice) the TMA engine copies the shifted NHWC window
 // [bn images x bh rows x bw cols] x 64 channels straight into 128B-swizzled shared memory; halo / padding pixels
 // come from TMA out-of-bounds zero fill (no im2col, no padded copy).  Products are "fp32-grade": every fp32
-// operand is pre-split into fp16 hi + lo and each k-slice issues hi*hi + hi*lo + lo*hi into one fp32 TMEM
+// operand is pre-split into fp16 hi + lo and each k-slice issues hi*hi + hi*lo + lo*hi into one fp32 register
 // accumulator (the dropped lo*lo term is ~2^-22 relative).
 //
 // Replaces, on the reference path, every torch.nn.Conv2d / 1x1 conv / bmm inside
 //   guided_diffusion/models.py:77-189 (ResnetBlock, AttnBlock), :36-74 (Up/Downsample)
 // which the reference dispatches to cuDNN / cuBLAS.
 //
-// CTA = 10 warps: warp 0 TMA producer, warp 1 UMMA issuer (+TMEM owner), warps 2-9 epilogue (TMEM -> regs -> HBM).
-// Persistent over output tiles; two TMEM accumulator stages so the epilogue of tile i overlaps the MMAs of tile i+1.
-// Three instantiations (picked per layer by the cost model in tc_make_launch, constants from profiles/r01_bn_sweep.md):
-//   <BN, false, false>  three instructions per k-step (hi*hi, hi*lo, lo*hi) into one accumulator;
-//   <BN, false, true>   DUAL: A_hi x [B_hi; B_lo] as one N = 2*BN instruction + A_lo x B_hi, two partial accumulators;
-//   <BN, true,  false>  PAIR: cluster of two CTAs, 256-row tcgen05.mma.cta_group::2, each CTA stages half of the B tile;
-//   <128, true, true>   PAIR + DUAL: 256 x 256 A_hi x [B_hi; B_lo] with the two planes held by the two CTAs + 256 x 128 A_lo x B_hi.
+// CTA = 9 warps: warps 0-7 are two consumer warpgroups (wgmma m64 x BN over rows 0-63 / 64-127 of the 128-pixel tile, then the
+// epilogue straight from the accumulator registers), warp 8 is the TMA producer.  Persistent over output tiles; the producer runs
+// ahead across tile boundaries, so the next tile's operands are in flight while the consumers run the epilogue.
+// Two orthogonal forms, chosen per layer in tc_make_launch:
+//   DUAL: the B_hi and B_lo planes of a stage are adjacent in shared memory, so ONE descriptor spans both and A_hi x [B_hi; B_lo] is
+//         a single m64 x 2BN instruction (accumulator columns [0, BN) = hi*hi, [BN, 2BN) = hi*lo); A_lo x B_hi follows with N = BN
+//         into the first half, and the epilogue adds the halves: two instructions and one read of the A_hi rows per k-step
+//         instead of three and two.
+//   PAIR: a cluster of two CTAs works on two M-adjacent tiles with the same N tile; each CTA TMA-loads its own A tile and HALF of
+//         the B tile, multicast into both CTAs' shared memory, so every weight row crosses L2 -> SM once per pair instead of twice.
+//         A stage may be refilled only when the consumers of BOTH CTAs have released it: each empty barrier counts the arrivals of
+//         the 16 consumer warps of the cluster.
+// And one with another A operand:
+//   GN:   fused GroupNorm + SiLU + fp16 split + 3x3 convolution (+ 1x1 shortcut as extra K blocks) on rows of >= 128 pixels.  Each
+//         consumer warpgroup reads its 64 pixels of the shifted fp32 rows itself, applies the per-(image, channel) affine of the
+//         normalisation (from the producer-side GroupNorm sums, plus scale-shift), SiLU, splits to fp16 hi / lo and stores them in
+//         the 128B-swizzled K-major layout TMA would have written; `fence.proxy.async` makes the generic-proxy stores visible to
+//         its wgmma.  The producer loads only the weights.  The fp16 planes of the activation never exist in HBM.
 #include "tc_gemm.cuh"
 
 #include <cstdlib>
-#include <type_traits>
 
 namespace ddnm {
 
 static constexpr int BM = 128;
-static constexpr int kTcThreads = 320;
+static constexpr int kConsumerThreads = 256;
+static constexpr int kTcThreads = kConsumerThreads + 32;
 static constexpr int BK = 64;                      // fp16 elements = 128 bytes = one swizzle row
 static constexpr int A_PLANE_BYTES = BM * BK * 2;  // 16 KiB
+static constexpr int kGnMaxC = 512;                // GN form: widest normalised input
 
-// PAIR: two CTAs of a cluster (one TPC) run ONE 256-row MMA (tcgen05 cta_group::2): each CTA stages its own 128-pixel A tile and
-// HALF of the B tile (BN/2 weight rows), the leader CTA issues the MMAs for both, every CTA drains its own 128 TMEM lanes.
-// Per MMA a CTA's shared memory now serves 128 + BN/2 operand rows instead of 128 + BN, which is what lets the Cout = 128
-// layers (BN = 128, the bulk of the celeba network) run the tensor pipe past the ~76 % the single-CTA form reaches.
-// DUAL (single-CTA, BN <= 128): two partial accumulators per TMEM stage, columns [0, BN) and [BN, 2BN), summed by the epilogue.
-// It lets hi*hi and hi*lo ride ONE N = 2*BN instruction (the hi and lo planes of the B tile are adjacent in shared memory, so
-// a single descriptor spans both): per 16-deep k-step the A_hi rows are read once instead of twice and 2 instructions are
-// issued instead of 3.
-// HALO (pairs, 3x3 stride 1 on rows >= 128 pixels wide): the A operand is staged ONCE per (64-channel slice, row offset dy) as a
-// halo row of 130 pixels (x0-1 .. x0+128) and feeds the three taps dx = -1, 0, +1 through UMMA descriptors whose start address is
-// shifted by one 128-byte operand row per tap (the hardware applies the 128B swizzle to the absolute address, so a shifted start
-// reads the right bytes: verified on the B200, profiles/r02_gn_fused_desc_mode.log).  The L2 -> shared-memory fill of A drops
-// 3x (it is 57 % of the 16.9 GB a 256 -> 128 layer pulls through the crossbar per launch, profiles/r02_forward_speedup.md).  A and B
-// then live in separate rings: A units of {hi, lo} x 136 rows, B stages of one tap's weights.
-template <int BN, bool PAIR, bool DUAL = false, bool HALO = false>
+template <int BN, bool DUAL>
 struct TcCfg {
-  static constexpr bool PD = PAIR && DUAL;                // both: see conv_tc_kernel's "PAIR + DUAL" note
-  static constexpr int B_ROWS = PAIR ? BN / 2 : BN;       // B rows staged by one CTA (plain PAIR)
-  static constexpr int B_PLANE_BYTES = B_ROWS * BK * 2;
-  // B regions of a stage: [X][Y].  plain / DUAL / PAIR: X = B_hi rows, Y = B_lo rows (B_PLANE_BYTES each).
-  // PAIR + DUAL: X = a FULL BN-row plane (B_hi in the leader, B_lo in the peer), Y = this CTA's BN/2-row half of B_hi.
-  static constexpr int BX_BYTES = PD ? BN * BK * 2 : B_PLANE_BYTES;
-  static constexpr int BY_BYTES = PD ? (BN / 2) * BK * 2 : B_PLANE_BYTES;
-  static constexpr int STAGE_BYTES = 2 * A_PLANE_BYTES + BX_BYTES + BY_BYTES;
-  static constexpr int STAGES = STAGE_BYTES <= 56 * 1024 ? 4 : (STAGE_BYTES <= 64 * 1024 ? 3 : 2);
-  // the epilogue's cross-warp combine buffer for the GroupNorm sums: 8 warps x BN/2 columns x float4; the PAIR + DUAL form has no
-  // room for it (4 x 56 KiB stages) and does not need it (contiguous tile ranges: one flush per CTA)
-  static constexpr bool COMBINE = !PD;
-  static constexpr int COMBINE_BYTES = COMBINE ? 8 * (BN / 2) * 16 : 0;
-  static constexpr int HA_PLANE = 136 * 128;              // 130 halo rows padded to 17 KiB (keeps the 1024-byte swizzle alignment)
-  static constexpr int HA_UNIT = 2 * HA_PLANE;            // hi + lo
-  static constexpr int HA_NA = 3;                         // A ring depth (units)
-  static constexpr int HB_STAGE = BX_BYTES + BY_BYTES;
-  static constexpr int HB_NB = PD ? 5 : 3;                // B ring depth (tap stages)
-  static constexpr int RING_BYTES = HALO ? HA_NA * HA_UNIT + HB_NB * HB_STAGE : STAGES * STAGE_BYTES;
-  static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + COMBINE_BYTES;
-  static constexpr int ACC_COLS = DUAL ? 2 * BN : BN;    // TMEM columns of one accumulator stage
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;
-  static_assert(TMEM_COLS <= 512 && SMEM_BYTES <= 227 * 1024, "TMEM / shared memory capacity");
+  static constexpr int B_PLANE_BYTES = BN * BK * 2;
+  static constexpr int STAGE_BYTES = 2 * A_PLANE_BYTES + 2 * B_PLANE_BYTES;   // A_hi, A_lo, B_hi, B_lo
+  static constexpr int STAGES = BN == 64 ? 4 : 3;
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  // GroupNorm sums of a tile: per-warp column partials (8 warps x BN x {sum, sumsq}) and the running (value, compensation) pairs
+  // of up to 4 images per tile x {sum, sumsq} x BN columns
+  static constexpr int PART_BYTES = 8 * BN * 8;
+  static constexpr int RUN_BYTES = 4 * 2 * BN * 8;
+  static constexpr int GN_BYTES = 2 * kGnMaxC * 4;   // GN form: per-channel scale and shift of the tile's image
+  static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + PART_BYTES + RUN_BYTES + GN_BYTES;
+  static constexpr int ACC = DUAL ? BN : BN / 2;     // fp32 accumulator registers per consumer thread (m64 x BN(x2) / 128 threads)
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory capacity");
 };
 
-template <int BN, bool PAIR, bool DUAL, bool HALO>
-__global__ void __launch_bounds__(HALO ? kTcThreads + 32 : kTcThreads, 1)
+// D[64 x N] (+)= A x B on the first N / 2 accumulator registers of d (the fragment of an m64 x N tile is a prefix of the one of a
+// wider tile, so the DUAL form's A_lo x B_hi accumulates into the hi*hi half of the m64 x 2BN accumulator)
+template <int N, int R>
+__device__ __forceinline__ void wgmma_tile(float (&d)[R], uint64_t a, uint64_t b, uint32_t accumulate) {
+  static_assert(N / 2 <= R, "accumulator too small");
+  if constexpr (N == 64) wgmma_m64n64k16(*reinterpret_cast<float(*)[32]>(&d[0]), a, b, accumulate);
+  else if constexpr (N == 128) wgmma_m64n128k16(*reinterpret_cast<float(*)[64]>(&d[0]), a, b, accumulate);
+  else wgmma_m64n256k16(*reinterpret_cast<float(*)[128]>(&d[0]), a, b, accumulate);
+}
+
+// GN form: 32 consecutive channels of one pixel (normalised + activated, or raw) -> fp16 hi / lo, stored as 4 swizzled 16-byte chunks
+// of row `row` (0..127) of the two 128-row A planes at a_hi / a_hi + A_PLANE_BYTES
+__device__ __forceinline__ void gn_store_row(uint8_t* a_hi, int row, int chunk0, const float (&v)[32]) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    uint4 h, l;
+    split2_f16(v[8 * q + 0], v[8 * q + 1], h.x, l.x);
+    split2_f16(v[8 * q + 2], v[8 * q + 3], h.y, l.y);
+    split2_f16(v[8 * q + 4], v[8 * q + 5], h.z, l.z);
+    split2_f16(v[8 * q + 6], v[8 * q + 7], h.w, l.w);
+    const int off = row * 128 + (((chunk0 + q) ^ (row & 7)) << 4);   // 128B swizzle: 16-byte chunk ^ (row mod 8)
+    *reinterpret_cast<uint4*>(a_hi + off) = h;
+    *reinterpret_cast<uint4*>(a_hi + A_PLANE_BYTES + off) = l;
+  }
+}
+
+template <int BN, bool PAIR, bool DUAL, bool GN>
+__global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant__ CUtensorMap tm_a0l,
                const __grid_constant__ CUtensorMap tm_a1h, const __grid_constant__ CUtensorMap tm_a1l,
-               const __grid_constant__ CUtensorMap tm_bh, const __grid_constant__ CUtensorMap tm_bl,
-               const __grid_constant__ CUtensorMap tm_b2, const TcParams p) {
-  // PAIR + DUAL (BN = 128: the Cout = 128 layers): A_hi x [B_hi; B_lo] as ONE 256 x 256 cta_group::2 instruction — the leader's
-  // smem supplies the B_hi plane (operand rows 0..127), the peer's the B_lo plane (rows 128..255) — then A_lo x B_hi as a 256 x 128
-  // instruction whose B halves (B_hi rows 0..63 / 64..127) sit in a third region Y of the stage (tm_b2: B_hi with a BN/2-row box).
-  static_assert(!HALO || PAIR, "the halo-row form exists for CTA pairs only");
-  using Cfg = TcCfg<BN, PAIR, DUAL, HALO>;
-  constexpr bool PD = Cfg::PD;
+               const __grid_constant__ CUtensorMap tm_bh, const __grid_constant__ CUtensorMap tm_bl, const TcParams p,
+               const TcGnArgs g) {
+  static_assert(!GN || !PAIR, "the GN form runs on single CTAs");
+  using Cfg = TcCfg<BN, DUAL>;
   constexpr int STAGES = Cfg::STAGES;
-  constexpr int NA = Cfg::HA_NA, NB = Cfg::HB_NB;
-  constexpr int NBAR = HALO ? 2 * NA + 2 * NB : 2 * STAGES;   // ring barriers in front of the accumulator ones
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + Cfg::RING_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  // HALO: A ring at the base, B ring behind it
-  const uint32_t a_ring = smem_base, b_ring = smem_base + NA * Cfg::HA_UNIT;
-  auto a_full = [&](int s) { return bar_base + 8u * s; };
-  auto a_empty = [&](int s) { return bar_base + 8u * (NA + s); };
-  auto b_full = [&](int s) { return bar_base + 8u * (2 * NA + s); };
-  auto b_empty = [&](int s) { return bar_base + 8u * (2 * NA + NB + s); };
-  auto tfull_bar = [&](int a) { return bar_base + 8u * (NBAR + a); };
-  auto tempty_bar = [&](int a) { return bar_base + 8u * (NBAR + 2 + a); };
-  const uint32_t tmem_slot = bar_base + 8u * (NBAR + 4);
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - smem_u32(smem_raw)));
+  uint8_t* stat_smem = smem_raw + (bar_base + 256u - smem_u32(smem_raw));
+  float2* part = reinterpret_cast<float2*>(stat_smem);                    // [warp][BN] {sum, sumsq} over the warp's 16 rows
+  float2* run = reinterpret_cast<float2*>(stat_smem + Cfg::PART_BYTES);   // [image slot][which][BN] {value, compensation}
+  float* gn_sc = reinterpret_cast<float*>(stat_smem + Cfg::PART_BYTES + Cfg::RUN_BYTES);   // GN: scale[kGnMaxC], shift[kGnMaxC]
+  float* gn_sh = gn_sc + kGnMaxC;
 
   pdl_prologue();
   const int warp = threadIdx.x >> 5;
@@ -109,60 +111,50 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
   const int KB = p.kb0 + p.kb1;
   const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
   const int total_tiles = m_tiles * p.n_tiles;
-  // p.deal == 0: tiles are dealt round-robin — at any moment the 148 CTAs work on 148 consecutive tiles (adjacent rows of one image).
+  // p.deal == 0: tiles are dealt round-robin — at any moment the resident CTAs work on consecutive tiles (adjacent rows of one image).
   // p.deal == 1 (layers with one N tile and GroupNorm sums to produce): every CTA owns a CONTIGUOUS range of tiles, so its tiles lie
   // in one or two images and the epilogue's running sums are flushed to the global accumulators once or twice per CTA instead
-  // of once per tile (with 128-tile images the round-robin order changes image at every step: 2048 same-address reductions per
-  // tile were costing the 128x128 layers +60 % — tests/diag epi_bench).
-  // PAIR: the scheduling unit is a pair of M-adjacent tiles sharing one N tile; CTA `rank` of the cluster owns tile 2*mp + rank.
+  // of once per tile.
+  // split-K (few tiles and a long K, i.e. the 8x8 level: 32-64 CTAs walking 72-144 k-blocks one after the other are
+  // latency-bound): p.split_k CTAs share a tile, each accumulates its own range of k-blocks and writes alpha * acc to its own
+  // partial buffer (p.out + ks * p.split_stride); splitk_reduce_kernel adds the partials in a fixed order, applies the epilogue
+  // terms and accumulates the GroupNorm sums — deterministic, no floating-point atomics
+  // PAIR: the scheduling unit is a pair of M-adjacent tiles sharing one N tile; CTA `rank` of the cluster owns tile 2 * mp + rank.
+  // Both CTAs walk the same units (each one's B halves feed the other).
   const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
-  // split-K (single-CTA launches with few tiles and a long K, i.e. the 8x8 level: 32-64 CTAs walking 72-144 k-blocks one after
-  // the other are latency-bound): p.split_k CTAs share a tile, each accumulates its own range of k-blocks and writes alpha * acc
-  // to its own partial buffer (p.out + ks * p.split_stride); splitk_reduce_kernel adds the partials in a fixed order, applies the
-  // epilogue terms and accumulates the GroupNorm sums — deterministic, no floating-point atomics
   const int n_units = PAIR ? total_tiles / 2 : total_tiles * p.split_k;
   const int n_workers = PAIR ? (int)(gridDim.x / 2) : (int)gridDim.x;
   const int worker = PAIR ? (int)cluster_id_x() : (int)blockIdx.x;
   const int unit_begin = p.deal ? (int)((long long)worker * n_units / n_workers) : worker;
   const int unit_end = p.deal ? (int)((long long)(worker + 1) * n_units / n_workers) : n_units;
   const int unit_step = p.deal ? 1 : n_workers;
-  auto k_lo = [&](int u) { return PAIR ? 0 : (int)((long long)(u % p.split_k) * KB / p.split_k); };
-  auto k_hi = [&](int u) { return PAIR ? KB : (int)((long long)(u % p.split_k + 1) * KB / p.split_k); };
+  auto k_lo = [&](int u) { return (int)((long long)(u % p.split_k) * KB / p.split_k); };
+  auto k_hi = [&](int u) { return (int)((long long)(u % p.split_k + 1) * KB / p.split_k); };
   auto tile_of = [&](int u) {
     if (!PAIR) return u / p.split_k;
     const int mp = u / p.n_tiles;
     return (2 * mp + (int)rank) * p.n_tiles + (u - mp * p.n_tiles);
   };
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_a0h);
-    tma_prefetch_desc(&tm_a0l);
+  if (warp == 8 && lane == 0) {
+    if (!GN) {
+      tma_prefetch_desc(&tm_a0h);
+      tma_prefetch_desc(&tm_a0l);
+    }
     tma_prefetch_desc(&tm_bh);
     tma_prefetch_desc(&tm_bl);
-    if (p.kb1) {
+    if (p.kb1 && !GN) {
       tma_prefetch_desc(&tm_a1h);
       tma_prefetch_desc(&tm_a1l);
     }
-    for (int s = 0; s < NBAR / 2; ++s) {   // full / empty pairs of the ring(s): one arrival each (expect_tx arrive / tcgen05.commit)
-      mbar_init(bar_base + 8u * (2 * s), 1);
-      mbar_init(bar_base + 8u * (2 * s + 1), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), PAIR ? 512 : 256);   // every epilogue thread (of both CTAs) arrives once per tile
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full_bar(s), 1);    // the producer's expect_tx arrive
+      mbar_init(empty_bar(s), PAIR ? 16 : 8);   // one arrive per consumer warp (of both CTAs of a pair)
     }
     mbar_fence_init();
   }
-  if (warp == 1) {
-    if (PAIR) tmem_alloc_pair(tmem_slot, Cfg::TMEM_COLS);
-    else tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (PAIR) cluster_sync_all();   // the peer's barriers exist before any remote arrive / TMA completion can reach them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
+  if (PAIR) cluster_sync_all();   // the peer's barriers exist before any multicast or remote arrive can reach them
+  else __syncthreads();
 
   auto decode = [&](int tile, int& n_idx, int& x0, int& y0, int& n0) {
     n_idx = tile % p.n_tiles;
@@ -176,64 +168,26 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
     n0 = tn * p.bn;
   };
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------ TMA producer ------------------------------------------------
     if (lane == 0) {
       uint32_t stage = 0, phase = 0;
-      // PAIR: both CTAs stage their halves; all bytes are credited to the LEADER's full barrier, which alone is armed
-      auto load4 = [&](uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3) {
-        if (PAIR) tma_load_4d_pair(dst, m, bar, c0, c1, c2, c3);
-        else tma_load_4d(dst, m, bar, c0, c1, c2, c3);
-      };
-      if constexpr (HALO) {
-        // weight (B) stages only: one per (unit, tap dx); the A halo rows come from warp 10
-        const int cb0 = p.cb0, upt = 3 * cb0 + p.kb1;
-        const uint32_t stage_tx = 2u * (uint32_t)Cfg::HB_STAGE;       // both CTAs' bytes land on the leader's barrier
-        for (int u = unit_begin; u < unit_end; u += unit_step) {
-          int n_idx, x0, y0, n0;
-          decode(tile_of(u), n_idx, x0, y0, n0);
-          for (int j = 0; j < upt; ++j) {
-            const bool side = j >= 3 * cb0;
-            const int c = side ? j - 3 * cb0 : j / 3;
-            const int dyi = side ? 0 : j - 3 * c;                     // 0..2 <-> dy = -1..1
-            const int ntap = side ? 1 : 3;
-            for (int dxi = 0; dxi < ntap; ++dxi) {
-              const int kb = side ? p.kb0 + c : ((dyi * 3 + dxi) * cb0 + c);
-              mbar_wait(b_empty(stage), phase ^ 1u);
-              const uint32_t sb = b_ring + stage * Cfg::HB_STAGE;
-              const uint32_t fb = b_full(stage);
-              if (leader) mbar_expect_tx(fb, stage_tx);
-              if (PD) {
-                tma_load_3d_pair(sb, rank == 0 ? &tm_bh : &tm_bl, fb, kb * BK, n_idx * BN, 0);
-                tma_load_3d_pair(sb + Cfg::BX_BYTES, &tm_b2, fb, kb * BK, n_idx * BN + (int)rank * (BN / 2), 0);
-              } else {
-                const int brow = n_idx * BN + (int)rank * Cfg::B_ROWS;
-                tma_load_3d_pair(sb, &tm_bh, fb, kb * BK, brow, 0);
-                tma_load_3d_pair(sb + Cfg::BX_BYTES, &tm_bl, fb, kb * BK, brow, 0);
-              }
-              if (++stage == (uint32_t)NB) {
-                stage = 0;
-                phase ^= 1u;
-              }
-            }
-          }
-        }
-      } else {
-      const uint32_t stage_tx = (PAIR ? 2u : 1u) * (uint32_t)(p.terms == 1 ? Cfg::STAGE_BYTES / 2 : Cfg::STAGE_BYTES);
+      const bool lo = p.terms != 1;
+      // GN: only the B planes arrive by TMA (the consumers write A themselves)
+      const uint32_t stage_tx = GN ? 2u * Cfg::B_PLANE_BYTES : (uint32_t)(lo ? Cfg::STAGE_BYTES : Cfg::STAGE_BYTES / 2);
       for (int u = unit_begin; u < unit_end; u += unit_step) {
-        const int tile = tile_of(u);
         int n_idx, x0, y0, n0;
-        decode(tile, n_idx, x0, y0, n0);
+        decode(tile_of(u), n_idx, x0, y0, n0);
         const int bz = p.b_batched == 1 ? n0 : 0;
-        const int brow = n_idx * BN + (int)rank * Cfg::B_ROWS;
         const int kb_lo = k_lo(u), kb_hi = k_hi(u);
         for (int kb = kb_lo; kb < kb_hi; ++kb) {
           mbar_wait(empty_bar(stage), phase ^ 1u);
           const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
+          const uint32_t sb = sa + 2 * A_PLANE_BYTES;
           const uint32_t fb = full_bar(stage);
-          if (leader) mbar_expect_tx(fb, stage_tx);
-          const bool lo = p.terms != 1;
-          if (kb < p.kb0) {
+          mbar_expect_tx(fb, stage_tx);
+          if (GN) {
+          } else if (kb < p.kb0) {
             const int tap = kb / p.cb0;
             const int c = (kb - tap * p.cb0) * BK;
             int cx = x0, cy = y0, cn = n0;
@@ -249,228 +203,188 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
               cx += dx >> 1;
               cn += ((dy & 1) * 2 + (dx & 1)) * p.phase_stride;
             }
-            load4(sa, &tm_a0h, fb, c, cx, cy, cn);
-            if (lo) load4(sa + A_PLANE_BYTES, &tm_a0l, fb, c, cx, cy, cn);
+            tma_load_4d(sa, &tm_a0h, fb, c, cx, cy, cn);
+            if (lo) tma_load_4d(sa + A_PLANE_BYTES, &tm_a0l, fb, c, cx, cy, cn);
           } else {
             const int c = (kb - p.kb0) * BK;
-            load4(sa, &tm_a1h, fb, c, x0, y0, n0);
-            if (lo) load4(sa + A_PLANE_BYTES, &tm_a1l, fb, c, x0, y0, n0);
+            tma_load_4d(sa, &tm_a1h, fb, c, x0, y0, n0);
+            if (lo) tma_load_4d(sa + A_PLANE_BYTES, &tm_a1l, fb, c, x0, y0, n0);
           }
-          if (PD) {
-            tma_load_3d_pair(sa + 2 * A_PLANE_BYTES, rank == 0 ? &tm_bh : &tm_bl, fb, kb * BK, n_idx * BN, bz);   // X: full plane
-            tma_load_3d_pair(sa + 2 * A_PLANE_BYTES + Cfg::BX_BYTES, &tm_b2, fb, kb * BK, n_idx * BN + (int)rank * (BN / 2), bz);
-          } else if (PAIR) {
-            tma_load_3d_pair(sa + 2 * A_PLANE_BYTES, &tm_bh, fb, kb * BK, brow, bz);
-            if (lo) tma_load_3d_pair(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES, &tm_bl, fb, kb * BK, brow, bz);
+          if (PAIR) {
+            // rows [rank * BN / 2, (rank + 1) * BN / 2) of the B tile, into both CTAs (each expects the whole stage)
+            const uint32_t half = (uint32_t)rank * (BN / 2) * 128u;
+            const int brow = n_idx * BN + (int)rank * (BN / 2);
+            tma_load_3d_multicast(sb + half, &tm_bh, fb, kb * BK, brow, 0, (uint16_t)3);
+            if (lo) tma_load_3d_multicast(sb + Cfg::B_PLANE_BYTES + half, &tm_bl, fb, kb * BK, brow, 0, (uint16_t)3);
           } else if (p.b_batched == 2) {
-            tma_load_4d(sa + 2 * A_PLANE_BYTES, &tm_bh, fb, kb * BK, n_idx * BN, y0, n0);
-            if (lo) tma_load_4d(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES, &tm_bl, fb, kb * BK, n_idx * BN, y0, n0);
+            tma_load_4d(sb, &tm_bh, fb, kb * BK, n_idx * BN, y0, n0);
+            if (lo) tma_load_4d(sb + Cfg::B_PLANE_BYTES, &tm_bl, fb, kb * BK, n_idx * BN, y0, n0);
           } else {
-            tma_load_3d(sa + 2 * A_PLANE_BYTES, &tm_bh, fb, kb * BK, n_idx * BN, bz);
-            if (lo) tma_load_3d(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES, &tm_bl, fb, kb * BK, n_idx * BN, bz);
+            tma_load_3d(sb, &tm_bh, fb, kb * BK, n_idx * BN, bz);
+            if (lo) tma_load_3d(sb + Cfg::B_PLANE_BYTES, &tm_bl, fb, kb * BK, n_idx * BN, bz);
           }
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1u;
           }
         }
-      }
-      }   // !HALO
-    }
-  } else if (HALO && warp == 10) {
-    // ------------------------------------------------ A halo-row producer (HALO) ----------------------------------
-    if constexpr (HALO) {
-      if (lane == 0) {
-        tma_prefetch_desc(&tm_a0h);
-        tma_prefetch_desc(&tm_a0l);
-        const int cb0 = p.cb0, upt = 3 * cb0 + p.kb1;
-        uint32_t ua = 0, aph = 0;
-        for (int u = unit_begin; u < unit_end; u += unit_step) {
-          int n_idx, x0, y0, n0;
-          decode(tile_of(u), n_idx, x0, y0, n0);
-          for (int j = 0; j < upt; ++j) {
-            const bool side = j >= 3 * cb0;
-            const int c = side ? j - 3 * cb0 : j / 3;
-            const int dyi = side ? 0 : j - 3 * c;
-            mbar_wait(a_empty(ua), aph ^ 1u);
-            const uint32_t sa = a_ring + ua * Cfg::HA_UNIT;
-            const uint32_t fb = a_full(ua);
-            // box bytes count in full even where the box hangs over the image (zero fill): 130 (main) / 128 (side) rows of 128 B,
-            // two planes, two CTAs
-            if (leader) mbar_expect_tx(fb, 4u * (uint32_t)(side ? 128 : 130) * 128u);
-            if (!side) {
-              // pixels x0-1 .. x0+128 of row y0 + dy -> operand rows 0..129; the conv's zero padding is the TMA out-of-bounds fill
-              tma_load_4d_pair(sa, &tm_a0h, fb, c * BK, x0 - 1, y0 + dyi - 1, n0);
-              tma_load_4d_pair(sa + Cfg::HA_PLANE, &tm_a0l, fb, c * BK, x0 - 1, y0 + dyi - 1, n0);
-            } else {
-              tma_load_4d_pair(sa, &tm_a1h, fb, c * BK, x0, y0, n0);
-              tma_load_4d_pair(sa + Cfg::HA_PLANE, &tm_a1l, fb, c * BK, x0, y0, n0);
-            }
-            if (++ua == (uint32_t)NA) {
-              ua = 0;
-              aph ^= 1u;
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------ UMMA issuer -------------------------------------------------
-    if (lane == 0 && leader) {
-      uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-      uint32_t h_ua = 0, h_aph = 0;   // HALO: A ring position
-      const uint64_t hi = (uint64_t)p.desc_hi << 32;
-      auto mma = [&](uint32_t d, uint64_t a, uint64_t b, uint32_t accumulate) {
-        if (PAIR) umma_f16_pair(d, a, b, p.idesc, accumulate);
-        else umma_f16(d, a, b, p.idesc, accumulate);
-      };
-      auto commit = [&](uint32_t bar) {
-        if (PAIR) umma_commit_pair(bar);
-        else umma_commit(bar);
-      };
-      for (int u = unit_begin; u < unit_end; u += unit_step) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * Cfg::ACC_COLS;
-        // DUAL: instruction descriptor of the N = 2*BN product A_hi x [B_hi; B_lo]
-        const uint32_t idesc_wide = (p.idesc & ~(0x3Fu << 17)) | ((uint32_t)((2 * BN) >> 3) << 17);
-        if constexpr (HALO) {
-          // `stage` / `phase` walk the B ring, ua / aph the A ring
-          const int cb0 = p.cb0, upt = 3 * cb0 + p.kb1;
-          bool first = true;
-          for (int j = 0; j < upt; ++j) {
-            const bool side = j >= 3 * cb0;
-            const int ntap = side ? 1 : 3;
-            mbar_wait(a_full(h_ua), h_aph);
-            tc_fence_after();
-            const uint32_t au = a_ring + h_ua * Cfg::HA_UNIT;
-            for (int dxi = 0; dxi < ntap; ++dxi) {
-              mbar_wait(b_full(stage), phase);
-              tc_fence_after();
-              // main units hold pixels x0-1 .. x0+128 in rows 0..129, tap dx reads rows dx+1 .. dx+128 (start address + dxi rows);
-              // side units hold pixels x0 .. x0+127 in rows 0..127
-              const uint32_t row_off = side ? 0u : (uint32_t)dxi * 128u;
-              const uint32_t ah = (((au + row_off) & 0x3FFFFu) >> 4) | (1u << 16);
-              const uint32_t al = (((au + Cfg::HA_PLANE + row_off) & 0x3FFFFu) >> 4) | (1u << 16);
-              const uint32_t sb = b_ring + stage * Cfg::HB_STAGE;
-              const uint32_t bx = ((sb & 0x3FFFFu) >> 4) | (1u << 16);
-              const uint32_t by = (((sb + Cfg::BX_BYTES) & 0x3FFFFu) >> 4) | (1u << 16);
-#pragma unroll
-              for (int k = 0; k < BK / 16; ++k) {
-                const uint32_t adv = 2u * k;
-                const uint32_t accum = (first && k == 0) ? 0u : 1u;
-                if (PD) {
-                  umma_f16_pair(d_tmem, hi | (ah + adv), hi | (bx + adv), idesc_wide, accum);   // [hi*hi | hi*lo]
-                  umma_f16_pair(d_tmem, hi | (al + adv), hi | (by + adv), p.idesc, 1u);         // lo*hi
-                } else {
-                  umma_f16_pair(d_tmem, hi | (ah + adv), hi | (bx + adv), p.idesc, accum);      // hi*hi
-                  umma_f16_pair(d_tmem, hi | (ah + adv), hi | (by + adv), p.idesc, 1u);         // hi*lo
-                  umma_f16_pair(d_tmem, hi | (al + adv), hi | (bx + adv), p.idesc, 1u);         // lo*hi
-                }
-              }
-              first = false;
-              umma_commit_pair(b_empty(stage));
-              if (++stage == (uint32_t)NB) {
-                stage = 0;
-                phase ^= 1u;
-              }
-            }
-            umma_commit_pair(a_empty(h_ua));   // the unit's rows (in both CTAs) may be overwritten once these MMAs have read them
-            if (++h_ua == (uint32_t)NA) {
-              h_ua = 0;
-              h_aph ^= 1u;
-            }
-          }
-          commit(tfull_bar(acc));
-          acc ^= 1u;
-          if (acc == 0) acc_phase ^= 1u;
-          continue;
-        }
-        const int kb_lo = k_lo(u), kb_hi = k_hi(u);
-        for (int kb = kb_lo; kb < kb_hi; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          // descriptor low word: start address >> 4 | LBO (unused for swizzled K-major, canonical value 1) << 16
-          const uint32_t ah = ((sa & 0x3FFFFu) >> 4) | (1u << 16);
-          const uint32_t al = (((sa + A_PLANE_BYTES) & 0x3FFFFu) >> 4) | (1u << 16);
-          const uint32_t bh = (((sa + 2 * A_PLANE_BYTES) & 0x3FFFFu) >> 4) | (1u << 16);
-          const uint32_t bl = (((sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES) & 0x3FFFFu) >> 4) | (1u << 16);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint32_t adv = 2u * k;  // 16 fp16 = 32 bytes = 2 x 16-byte units inside the swizzle row
-            if (PD) {
-              // region X of the two CTAs forms [B_hi; B_lo]; region Y holds the B_hi halves of the 256 x 128 product
-              const uint32_t by = (((sa + 2 * A_PLANE_BYTES + Cfg::BX_BYTES) & 0x3FFFFu) >> 4) | (1u << 16);
-              umma_f16_pair(d_tmem, hi | (ah + adv), hi | (bh + adv), idesc_wide, (uint32_t)(kb != kb_lo || k != 0));
-              umma_f16_pair(d_tmem, hi | (al + adv), hi | (by + adv), p.idesc, 1u);
-            } else if (DUAL && p.terms != 1) {
-              // columns [0,BN) += A_hi*B_hi, [BN,2BN) += A_hi*B_lo in one instruction; then [0,BN) += A_lo*B_hi
-              umma_f16(d_tmem, hi | (ah + adv), hi | (bh + adv), idesc_wide, (uint32_t)(kb != kb_lo || k != 0));
-              umma_f16(d_tmem, hi | (al + adv), hi | (bh + adv), p.idesc, 1u);
-            } else {
-              mma(d_tmem, hi | (ah + adv), hi | (bh + adv), (uint32_t)(kb != kb_lo || k != 0));
-              if (p.terms != 1) {
-                mma(d_tmem, hi | (ah + adv), hi | (bl + adv), 1u);
-                mma(d_tmem, hi | (al + adv), hi | (bh + adv), 1u);
-              }
-            }
-          }
-          commit(empty_bar(stage));  // smem slot (of both CTAs) reusable once these MMAs have read it
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        commit(tfull_bar(acc));  // accumulator complete -> epilogue (of both CTAs)
-        acc ^= 1u;
-        if (acc == 0) acc_phase ^= 1u;
       }
     }
   } else {
-    // ------------------------------------------------ epilogue ----------------------------------------------------
-    // 8 epilogue warps: warp w may touch TMEM lanes 32*(w%4)..+31; the two warps sharing a lane quarter split the columns.
-    // Per tile a warp handles NCH chunks of 32 columns.  Latency is what the epilogue is made of (ncu: the warps sit on the long
-    // scoreboard), so nothing that does not depend on the accumulator waits for it: the residual rows of a chunk are requested one
-    // chunk earlier (across the tile boundary too, i.e. while the MMAs of the tile are still running), both partial accumulators are
-    // read with one wait, the TMEM stage goes back to the MMA issuer right after the last read, and rows move as 32-byte vectors
-    // (whole sectors per thread: half the LSU instructions of 16-byte accesses and no partial-sector writes).
-    const int ew = warp & 3;
-    const int chalf = (warp - 2) >> 2;
-    constexpr int CW = BN / 2;      // columns per epilogue warp
-    constexpr int NCH = CW / 32;    // 32-column chunks per warp and tile
-    const int r = ew * 32 + lane;
-    const int xi = r % p.bw;
-    const int yi = (r / p.bw) % p.bh;
-    const int ni = r / (p.bw * p.bh);
-    uint32_t acc = 0, acc_phase = 0;
-    // running GroupNorm sums of this warp's columns over the CTA's consecutive tiles of one image, as (value, compensation) pairs:
-    // a contiguous tile range accumulates tens of tiles before a flush, and the two-sum keeps that as exact as one flush per tile
-    float run_s[NCH], run_q[NCH], cmp_s[NCH], cmp_q[NCH];
-#pragma unroll
-    for (int ch = 0; ch < NCH; ++ch) {
-      run_s[ch] = 0.f;
-      run_q[ch] = 0.f;
-      cmp_s[ch] = 0.f;
-      cmp_q[ch] = 0.f;
+  // ------------------------------------------------ consumers: wgmma + epilogue ------------------------------------------------
+  // warpgroup wg owns tile rows [64 wg, 64 wg + 64); in the m64 accumulator fragment a thread holds, for every 8-column group j,
+  // columns 8j + 2(lane % 4) + {0, 1} of rows r0 = 16 warp + lane / 4 (d[4j], d[4j+1]) and r0 + 8 (d[4j+2], d[4j+3])
+  const int wg = warp >> 2;
+  const uint32_t a_row_off = (uint32_t)wg * 64u * 128u;
+  const int r0 = warp * 16 + (lane >> 2);
+  const int cq = (lane & 3) * 2;
+  const int tid = threadIdx.x;
+  const int ppi = p.bw * p.bh;                // pixels (tile rows) per image
+  const int wpi = ppi >= 128 ? 8 : ppi / 16;  // warps per image slot of the tile
+  uint32_t stage = 0, phase = 0;
+  if (p.stats) {
+    for (int i = tid; i < 4 * 2 * BN; i += kConsumerThreads) run[i] = make_float2(0.f, 0.f);
+  }
+  float d[Cfg::ACC];
+  const bool dual = DUAL && p.terms != 1;
+  int gn_image = -1;   // GN: image whose scale / shift are in gn_sc / gn_sh
+  auto release = [&](int s) {
+    if (lane == 0) {
+      mbar_arrive(empty_bar(s));
+      if (PAIR) mbar_arrive_cluster(empty_bar(s), rank ^ 1u);
     }
-    const bool dual_sum = DUAL && p.terms != 1;
-    struct Tile {
-      float* orow;
-      const float* rrow;      // residual source row (same pixel / nearest-upsampled / top-left of the 2x2 block to average)
-      const float* crow;
-      int n_idx, img_w;
-      bool valid;
-    };
-    auto setup = [&](int u, Tile& t) {
-      int x0, y0, n0;
-      decode(tile_of(u), t.n_idx, x0, y0, n0);
+  };
+  for (int u = unit_begin; u < unit_end; u += unit_step) {
+    const int kb_lo = k_lo(u), kb_hi = k_hi(u);
+    int prev = -1;
+    int t_nidx, t_x0, t_y0, t_n0;   // this tile's coordinates (GN: pixels of the A rows)
+    decode(tile_of(u), t_nidx, t_x0, t_y0, t_n0);
+    if constexpr (GN) {
+      if (g.norm && t_n0 != gn_image && t_n0 < p.N) {
+        // per-channel affine of this image's normalisation, as gn_apply_kernel computes it (double sums, rstd in fp32)
+        named_bar_sync(1, kConsumerThreads);   // both warpgroups are done with the previous image's table
+        const int cpg = g.C / g.groups;
+        const double cnt = (double)p.H * p.W * cpg;
+        for (int c = tid; c < g.C; c += kConsumerThreads) {
+          const int g0 = (c / cpg) * cpg;
+          double s1 = 0, s2 = 0;
+          for (int j = 0; j < cpg; ++j) {
+            s1 += stat_value(g.st[((size_t)t_n0 * g.st_ld + g0 + j) * 2]);
+            s2 += stat_value(g.st[((size_t)t_n0 * g.st_ld + g0 + j) * 2 + 1]);
+          }
+          const double mean = s1 / cnt;
+          double var = s2 / cnt - mean * mean;
+          var = var < 0 ? 0 : var;
+          const float rstd = (float)(1.0 / sqrt(var + (double)g.eps));
+          float a = rstd * g.gamma[c];
+          float b = g.beta[c] - (float)mean * a;
+          if (g.ss) {  // h = norm(h) * (1 + scale) + shift
+            const float one_plus = 1.0f + g.ss[(size_t)t_n0 * g.ss_ld + c];
+            a *= one_plus;
+            b = fmaf(b, one_plus, g.ss[(size_t)t_n0 * g.ss_ld + g.C + c]);
+          }
+          gn_sc[c] = a;
+          gn_sh[c] = b;
+        }
+        named_bar_sync(1, kConsumerThreads);
+        gn_image = t_n0;
+      }
+    }
+    for (int kb = kb_lo; kb < kb_hi; ++kb) {
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
+      if constexpr (GN) {
+        // this warpgroup's 64 A rows: pixel x0 + row of row y0 (tiles are 128 pixels of one row), shifted by the tap
+        const int rr = (tid & 127) >> 1, half = tid & 1, row = wg * 64 + rr;
+        float v[32];
+        bool valid = t_n0 < p.N;
+        const float* src;
+        if (kb < p.kb0) {
+          const int tap = kb / p.cb0, c0 = (kb - tap * p.cb0) * BK + half * 32;
+          const int yy = t_y0 + tap / 3 - 1, xx = t_x0 + row + tap % 3 - 1;
+          valid = valid && yy >= 0 && yy < p.H && xx >= 0 && xx < p.W;
+          src = g.x + (((long long)t_n0 * p.H + yy) * p.W + xx) * g.x_ld + c0;
+          if (valid) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+              const float4 f = __ldg(reinterpret_cast<const float4*>(src + 4 * q));
+              v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
+            }
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              if (g.norm) v[j] = fmaf(v[j], gn_sc[c0 + j], gn_sh[c0 + j]);
+              if (g.silu) v[j] = swishf_fast(v[j]);
+            }
+          }
+        } else {   // the 1x1 shortcut's raw input at the output pixel
+          const int c0 = (kb - p.kb0) * BK + half * 32;
+          src = g.xs + (((long long)t_n0 * p.H + t_y0) * p.W + t_x0 + row) * g.xs_ld + c0;
+          if (valid) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+              const float4 f = __ldg(reinterpret_cast<const float4*>(src + 4 * q));
+              v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
+            }
+          }
+        }
+        if (!valid) {   // the convolution's zero padding (of the activated tensor) and rows past the batch
+#pragma unroll
+          for (int j = 0; j < 32; ++j) v[j] = 0.f;
+        }
+        gn_store_row(smem_raw + (sa - smem_u32(smem_raw)), row, half * 4, v);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to wgmma
+        named_bar_sync(2 + wg, 128);
+      }
+      const uint64_t ah = wgmma_desc_sw128(sa + a_row_off);
+      const uint64_t al = wgmma_desc_sw128(sa + A_PLANE_BYTES + a_row_off);
+      const uint64_t bh = wgmma_desc_sw128(sa + 2 * A_PLANE_BYTES);
+      const uint64_t bl = wgmma_desc_sw128(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t adv = 2u * k;   // 16 fp16 = 32 bytes = 2 x 16-byte units inside the swizzle row
+        const uint32_t acc = (uint32_t)(kb != kb_lo || k != 0);
+        if (dual) {
+          wgmma_tile<DUAL ? 2 * BN : BN>(d, ah + adv, bh + adv, acc);   // [hi*hi | hi*lo]: bh spans both adjacent planes
+          wgmma_tile<BN>(d, al + adv, bh + adv, 1u);        // lo*hi into the hi*hi half
+        } else {
+          wgmma_tile<BN>(d, ah + adv, bh + adv, acc);
+          if (p.terms != 1) {
+            wgmma_tile<BN>(d, ah + adv, bl + adv, 1u);
+            wgmma_tile<BN>(d, al + adv, bh + adv, 1u);
+          }
+        }
+      }
+      wgmma_commit();
+      // the previous k-block's group has completed once at most this one is pending: its stage goes back to the producer
+      wgmma_wait<1>();
+      if (prev >= 0) release(prev);
+      prev = (int)stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1u;
+      }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0) release(prev);
+
+    // ---- epilogue: rows r0 and r0 + 8 of this tile, 2 adjacent columns per 8-column group ----
+    int n_idx, x0, y0, n0;
+    decode(tile_of(u), n_idx, x0, y0, n0);
+    const int split_off = PAIR ? 0 : u % p.split_k;
+    float* orow[2];
+    const float* rrow[2];
+    const float* crow[2];
+    bool valid[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = r0 + 8 * h;
+      const int xi = r % p.bw, yi = (r / p.bw) % p.bh, ni = r / ppi;
       const int n = n0 + ni;
-      t.valid = n < p.N;
-      t.img_w = n0 + (ew * 32) / (p.bw * p.bh);
-      t.orow = p.out + (long long)n * p.out_sn + (long long)(y0 + yi) * p.out_sy + (long long)(x0 + xi) * p.out_sx + t.n_idx * BN +
-               (PAIR ? 0ll : (long long)(u % p.split_k) * p.split_stride);
-      t.rrow = nullptr;
+      valid[h] = n < p.N;
+      orow[h] = p.out + (long long)n * p.out_sn + (long long)(y0 + yi) * p.out_sy + (long long)(x0 + xi) * p.out_sx + n_idx * BN +
+                (long long)split_off * p.split_stride;
+      rrow[h] = nullptr;
       if (p.residual) {
         // same pixel, nearest-upsampled (x_upd of ResBlock(up=True), unet.py:240) or the 2x2 average of a twice-as-large map
         // (ResBlock(down=True))
@@ -478,176 +392,100 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
         if (p.res_mode == 0) rp = ((long long)n * p.H + (y0 + yi)) * p.W + (x0 + xi);
         else if (p.res_mode == 1) rp = ((long long)n * (p.H >> 1) + ((y0 + yi) >> 1)) * (p.W >> 1) + ((x0 + xi) >> 1);
         else rp = ((long long)n * (2 * p.H) + 2 * (y0 + yi)) * (2 * p.W) + 2 * (x0 + xi);
-        t.rrow = p.residual + rp * p.ldr + t.n_idx * BN;
+        rrow[h] = p.residual + rp * p.ldr + n_idx * BN;
       }
-      t.crow = p.chanadd ? p.chanadd + (long long)n * p.ca_ld + t.n_idx * BN : nullptr;
-    };
-    // residual columns [c0, c0 + 32) of a tile's row (zeros if there is none)
-    auto load_res = [&](const Tile& t, int c0, float (&rv)[32]) {
-      if (t.rrow != nullptr && t.valid) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) ldg_f32x8(t.rrow + c0 + 8 * j, &rv[8 * j]);
-        if (p.res_mode == 2) {
-          const long long r_dx = p.ldr, r_dy = (long long)2 * p.W * p.ldr;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float q1[8], q2[8], q3[8];
-            ldg_f32x8(t.rrow + r_dx + c0 + 8 * j, q1);
-            ldg_f32x8(t.rrow + r_dy + c0 + 8 * j, q2);
-            ldg_f32x8(t.rrow + r_dy + r_dx + c0 + 8 * j, q3);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) rv[8 * j + i] = ((rv[8 * j + i] + q1[i]) + (q2[i] + q3[i])) * 0.25f;
-          }
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) rv[j] = 0.f;
-      }
-    };
-    // the tile loop, compiled twice: with a residual (its rows are requested one chunk ahead and live in 2 x 32 registers) and
-    // without (no such registers, no additions of zeros)
-    auto tile_loop = [&](auto res_tag) {
-    constexpr bool HAS_RES = decltype(res_tag)::value;
-    Tile cur, nxt;
-    float rvn[HAS_RES ? 32 : 1];   // residual of the NEXT chunk to be processed, in flight
-    if (unit_begin < unit_end) {
-      setup(unit_begin, cur);
-      if constexpr (HAS_RES) load_res(cur, chalf * CW, rvn);
+      crow[h] = p.chanadd ? p.chanadd + (long long)n * p.ca_ld + n_idx * BN : nullptr;
     }
-    for (int u = unit_begin; u < unit_end; u += unit_step) {
-      const bool has_next = u + unit_step < unit_end;
-      if (has_next) setup(u + unit_step, nxt);
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tc_fence_after();
-      const uint32_t t0 = tmem_base + ((uint32_t)(ew * 32) << 16) + acc * Cfg::ACC_COLS;
 #pragma unroll
-      for (int ch = 0; ch < NCH; ++ch) {
-        const int c0 = chalf * CW + ch * 32;
-        float rv[HAS_RES ? 32 : 1];
-        if constexpr (HAS_RES) {
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = 8 * j + cq;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) rv[j] = rvn[j];
-        }
-        uint32_t v[32], v2[32];
-        tmem_ld32(t0 + c0, v);
-        if (dual_sum) tmem_ld32(t0 + BN + c0, v2);   // the hi*lo partial sums kept in the stage's second half
-        if constexpr (HAS_RES) {
-          if (ch + 1 < NCH) load_res(cur, c0 + 32, rvn);
-          else if (has_next) load_res(nxt, chalf * CW, rvn);
-        }
-        tmem_ld_wait();
-        if (ch == NCH - 1) {
-          // every accumulator column this warp owns is in registers: hand the TMEM stage back before the arithmetic and the stores
-          tc_fence_before();
-          if (PAIR) mbar_arrive_leader(tempty_bar(acc));
-          else mbar_arrive(tempty_bar(acc));
-        }
-        float ov[32];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 cv = cur.crow ? __ldg(reinterpret_cast<const float4*>(cur.crow + c0 + 4 * j)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          float a0 = __uint_as_float(v[4 * j + 0]), a1 = __uint_as_float(v[4 * j + 1]);
-          float a2 = __uint_as_float(v[4 * j + 2]), a3 = __uint_as_float(v[4 * j + 3]);
-          if (dual_sum) {
-            a0 += __uint_as_float(v2[4 * j + 0]);
-            a1 += __uint_as_float(v2[4 * j + 1]);
-            a2 += __uint_as_float(v2[4 * j + 2]);
-            a3 += __uint_as_float(v2[4 * j + 3]);
+      for (int h = 0; h < 2; ++h) {
+        float a0 = d[4 * j + 2 * h], a1 = d[4 * j + 2 * h + 1];
+        if constexpr (DUAL) {
+          if (dual) {   // + the hi*lo partial sums of the same columns, kept BN columns further on
+            a0 += d[4 * (j + BN / 8) + 2 * h];
+            a1 += d[4 * (j + BN / 8) + 2 * h + 1];
           }
-          ov[4 * j + 0] = cur.valid ? p.alpha * a0 + cv.x + (HAS_RES ? rv[4 * j + 0] : 0.f) : 0.f;
-          ov[4 * j + 1] = cur.valid ? p.alpha * a1 + cv.y + (HAS_RES ? rv[4 * j + 1] : 0.f) : 0.f;
-          ov[4 * j + 2] = cur.valid ? p.alpha * a2 + cv.z + (HAS_RES ? rv[4 * j + 2] : 0.f) : 0.f;
-          ov[4 * j + 3] = cur.valid ? p.alpha * a3 + cv.w + (HAS_RES ? rv[4 * j + 3] : 0.f) : 0.f;
         }
-        if (cur.valid) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) stg_f32x8(cur.orow + c0 + 8 * j, &ov[8 * j]);
+        float v0 = p.alpha * a0, v1 = p.alpha * a1;
+        if (crow[h] && valid[h]) {
+          const float2 cv = __ldg(reinterpret_cast<const float2*>(crow[h] + c));
+          v0 += cv.x;
+          v1 += cv.y;
         }
-        if (p.stats) {
-          // GroupNorm statistics of the tile: transpose-reduce the 32 rows x 32 columns this warp holds so that lane L
-          // ends with the column-(c0+L) sum and sum of squares over the warp's 32 pixels (31 shuffles per statistic)
-          float sq[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) sq[j] = ov[j] * ov[j];
-#pragma unroll
-          for (int k = 16; k >= 1; k >>= 1) {
-            const bool up = (lane & k) != 0;
-#pragma unroll
-            for (int i = 0; i < k; ++i) {
-              const float keep_s = up ? ov[i + k] : ov[i], send_s = up ? ov[i] : ov[i + k];
-              const float keep_q = up ? sq[i + k] : sq[i], send_q = up ? sq[i] : sq[i + k];
-              ov[i] = keep_s + __shfl_xor_sync(0xffffffffu, send_s, k);
-              sq[i] = keep_q + __shfl_xor_sync(0xffffffffu, send_q, k);
-            }
+        if (rrow[h] && valid[h]) {
+          float2 rv = __ldg(reinterpret_cast<const float2*>(rrow[h] + c));
+          if (p.res_mode == 2) {
+            const long long r_dx = p.ldr, r_dy = (long long)2 * p.W * p.ldr;
+            const float2 q1 = __ldg(reinterpret_cast<const float2*>(rrow[h] + r_dx + c));
+            const float2 q2 = __ldg(reinterpret_cast<const float2*>(rrow[h] + r_dy + c));
+            const float2 q3 = __ldg(reinterpret_cast<const float2*>(rrow[h] + r_dy + r_dx + c));
+            rv.x = ((rv.x + q1.x) + (q2.x + q3.x)) * 0.25f;
+            rv.y = ((rv.y + q1.y) + (q2.y + q3.y)) * 0.25f;
           }
-          two_sum_acc(run_s[ch], cmp_s[ch], ov[0]);
-          two_sum_acc(run_q[ch], cmp_q[ch], sq[0]);
+          v0 += rv.x;
+          v1 += rv.y;
         }
+        if (!valid[h]) v0 = v1 = 0.f;
+        d[4 * j + 2 * h] = v0;
+        d[4 * j + 2 * h + 1] = v1;
+        if (valid[h]) *reinterpret_cast<float2*>(orow[h] + c) = make_float2(v0, v1);
       }
-      if (p.stats) {
-        // the warp's 32 rows lie in one image (>= 32 pixels per image): keep running sums while consecutive tiles stay in
-        // the same image / channel block (the tile -> CTA map is static, so these fp32 partial sums are the same every run),
-        // flush with one order-independent fixed-point add pair per column otherwise
-        if (!has_next || nxt.img_w != cur.img_w || nxt.n_idx != cur.n_idx) {
-          if constexpr (Cfg::COMBINE) {
-            // the warps of this column half whose rows lie in the same image (4, or 2 on 8x8 maps) first add their sums in shared
-            // memory, in a fixed order: 4x fewer same-address reductions reach L2 (with several N tiles the round-robin tile order
-            // changes image or channel block at every tile, so this runs once per tile)
-            const int wpi = min(4, (p.bw * p.bh) >> 5);          // warps per image
-            const int pos = ew % wpi, first = ew - pos;
-            float4* cb = reinterpret_cast<float4*>(smem_raw + (bar_base + 256u - smem_u32(smem_raw))) + (size_t)chalf * 4 * CW;
-#pragma unroll
-            for (int ch = 0; ch < NCH; ++ch) cb[ew * CW + ch * 32 + lane] = make_float4(run_s[ch], cmp_s[ch], run_q[ch], cmp_q[ch]);
-            named_bar_sync(1 + chalf, 128);
-            if (cur.img_w < p.N) {
-              for (int slot = pos * 32 + lane; slot < 2 * CW; slot += wpi * 32) {
-                const int which = slot >= CW ? 1 : 0, col = slot - which * CW;
-                float sum = 0.f, comp = 0.f;
-                for (int w = 0; w < wpi; ++w) {
-                  const float4 t = cb[(first + w) * CW + col];
-                  two_sum_acc(sum, comp, which ? t.z : t.x);
-                  two_sum_acc(sum, comp, which ? t.w : t.y);
-                }
-                stat_add(p.stats + ((size_t)cur.img_w * p.st_ld + cur.n_idx * BN + chalf * CW + col) * 2 + which, sum + comp);
-              }
-            }
-            named_bar_sync(1 + chalf, 128);
-          } else if (cur.img_w < p.N) {
-#pragma unroll
-            for (int ch = 0; ch < NCH; ++ch) {
-              StatAcc* d = p.stats + ((size_t)cur.img_w * p.st_ld + cur.n_idx * BN + chalf * CW + ch * 32 + lane) * 2;
-              stat_add(d, run_s[ch]);        // integer accumulation: the total is independent of the arrival order
-              stat_add(d, cmp_s[ch]);
-              stat_add(d + 1, run_q[ch]);
-              stat_add(d + 1, cmp_q[ch]);
-            }
-          }
-#pragma unroll
-          for (int ch = 0; ch < NCH; ++ch) {
-            run_s[ch] = 0.f;
-            run_q[ch] = 0.f;
-            cmp_s[ch] = 0.f;
-            cmp_q[ch] = 0.f;
-          }
-        }
-      }
-      cur = nxt;
-      acc ^= 1u;
-      if (acc == 0) acc_phase ^= 1u;
     }
-    };
-    if (p.residual) tile_loop(std::true_type{});
-    else tile_loop(std::false_type{});
+    if (p.stats) {
+      // GroupNorm statistics of the tile.  (1) per warp: the column sums over its 16 rows (one image: >= 32 pixels per image),
+      // reduced across the 8 lanes that share a column pair; (2) per image slot: the warps of that image added in a fixed order
+      // into running (value, compensation) pairs that persist while consecutive tiles of this CTA stay in the same image and
+      // channel block (the tile -> CTA map is static, so these fp32 partial sums are the same every run); (3) flushed with one
+      // order-independent fixed-point add per value otherwise
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float a = d[4 * j + e], b = d[4 * j + 2 + e];
+          float s = a + b, q = a * a + b * b;
+#pragma unroll
+          for (int k = 4; k <= 16; k <<= 1) {
+            s += __shfl_xor_sync(0xffffffffu, s, k);
+            q += __shfl_xor_sync(0xffffffffu, q, k);
+          }
+          if (lane < 4) part[warp * BN + 8 * j + cq + e] = make_float2(s, q);
+        }
+      }
+      named_bar_sync(1, kConsumerThreads);
+      const int nslots = 8 / wpi;
+      bool flush = true;
+      if (u + unit_step < unit_end) {
+        int nn_idx, nx0, ny0, nn0;
+        decode(tile_of(u + unit_step), nn_idx, nx0, ny0, nn0);
+        flush = nslots > 1 || nn0 != n0 || nn_idx != n_idx;
+      }
+      for (int i = tid; i < 2 * BN; i += kConsumerThreads) {
+        const int which = i / BN, col = i - which * BN;
+        for (int g = 0; g < nslots; ++g) {
+          float2& acc = run[(g * 2 + which) * BN + col];
+          for (int w = g * wpi; w < (g + 1) * wpi; ++w) {
+            const float2 pv = part[w * BN + col];
+            two_sum_acc(acc.x, acc.y, which ? pv.y : pv.x);
+          }
+          if (flush) {
+            const int n = n0 + g;
+            if (n < p.N) {
+              StatAcc* dst = p.stats + ((size_t)n * p.st_ld + n_idx * BN + col) * 2 + which;
+              stat_add(dst, acc.x);   // integer accumulation: the total is independent of the arrival order
+              stat_add(dst, acc.y);
+            }
+            acc = make_float2(0.f, 0.f);
+          }
+        }
+      }
+      named_bar_sync(1, kConsumerThreads);   // part[] is rewritten by the next tile
+    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (PAIR) cluster_sync_all();   // the leader's MMAs / commits no longer touch the peer's smem, TMEM or barriers
-  if (warp == 1) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair(tmem_base, Cfg::TMEM_COLS);
-    else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
   }
+  __syncwarp();                   // the producer warp's lane 0 leaves its loop before the aligned cluster barrier
+  if (PAIR) cluster_sync_all();   // no multicast or remote arrive may reach a CTA that has exited
 }
 
 // -------------------------------------------------------------------------------------------------------------------
@@ -690,46 +528,30 @@ static CUtensorMap make_map_f16(const void* base, int rank, const uint64_t* dims
   return m;
 }
 
-// 3D map over a K-major [Cout][Ktot] fp16 weight matrix with a (64, box_rows, 1) box (used by the fused GroupNorm convolution)
-CUtensorMap tc_make_weight_map(const __half* w, int Ktot, int Cout, int box_rows) {
-  const uint64_t bd[3] = {(uint64_t)Ktot, (uint64_t)Cout, 1u};
-  const uint32_t bbox[3] = {(uint32_t)BK, (uint32_t)box_rows, 1u};
-  return make_map_f16(w, 3, bd, bbox);
-}
-
-static uint32_t g_desc_hi_override = 0, g_idesc_xor = 0;
 static int g_terms = 3;
 void tc_set_terms(int terms) {
   DDNM_CHECK(terms == 1 || terms == 3, "terms must be 1 or 3");
   g_terms = terms;
 }
 int tc_get_terms() { return g_terms; }
-static int g_pair_mode = -1;   // -1: cost model decides (default), 0: never, 1: CTA pairs wherever legal
-static double g_pair_tkb[2] = {1300.0, 1770.0};   // clocks per k-block of the pair kernel at BN = 128 / 256 (sweep)
-static int g_pair_dual = 1;                         // 1 (default): pairs at BN = 128 use the PAIR + DUAL form
-static double g_pair_dual_tkb = 935.0;              // measured: 3-6 % under DUAL's 1000 on the 256x256 / 128x128 layers
-void tc_debug_pair_dual(int on) { g_pair_dual = on; }
-void tc_debug_pair_mode(int mode) {
-  DDNM_CHECK(mode == -1 || mode == 0 || mode == 1, "pair mode must be -1 (cost model), 0 (off) or 1 (wherever legal)");
-  g_pair_mode = mode;
-}
-static int g_dual_mode = 1;   // 1: single-CTA launches with BN <= 128 use the DUAL kernel (default), 0: never
-void tc_debug_dual_mode(int mode) { g_dual_mode = mode; }
 static int g_force_bn = 0;
 void tc_debug_force_bn(int bn) {
-  DDNM_CHECK(bn == 0 || bn == 64 || bn == 128 || bn == 256, "BN must be 0 (heuristic), 64, 128 or 256");
+  DDNM_CHECK(bn == 0 || bn == 64 || bn == 128, "BN must be 0 (heuristic), 64 or 128");
   g_force_bn = bn;
 }
-static int g_halo = [] { const char* v = std::getenv("DDNM_HALO"); return v && *v ? std::atoi(v) : 1; }();
-void tc_debug_halo(int on) { g_halo = on; }
+static int g_pair_mode = -1;   // -1: default (no pairs, see tc_make_launch), 0: never, 1: CTA pairs wherever legal
+void tc_debug_pair_mode(int mode) {
+  DDNM_CHECK(mode == -1 || mode == 0 || mode == 1, "pair mode must be -1 (default rule), 0 (off) or 1 (wherever legal)");
+  g_pair_mode = mode;
+}
+static int g_dual_mode = 1;    // 1: single-CTA launches use the DUAL form (default), 0: never
+void tc_debug_dual_mode(int mode) { g_dual_mode = mode; }
+static int g_pair_dual = 1;    // 1: CTA pairs use the DUAL form as well (default), 0: the plain three-instruction pair form
+void tc_debug_pair_dual(int on) { g_pair_dual = on; }
 static int g_deal = -1;
 void tc_debug_deal(int mode) {
   DDNM_CHECK(mode >= -1 && mode <= 1, "deal mode must be -1 (default rule), 0 (round-robin) or 1 (contiguous ranges)");
   g_deal = mode;
-}
-void tc_debug_override(uint32_t desc_hi, uint32_t idesc_xor) {
-  g_desc_hi_override = desc_hi;
-  g_idesc_xor = idesc_xor;
 }
 
 TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1, const __half* w_hi, const __half* w_lo,
@@ -750,45 +572,23 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
   p.tiles_x = out.W / p.bw;
   p.tiles_y = out.H / p.bh;
   p.tiles_n = cdiv(out.N, p.bn);
-  // Tile shape by a small cost model fitted to the B200 sweep in profiles/r01_bn_sweep.md.  Every configuration turned out to be
-  // paced by SHARED-MEMORY bandwidth, not by the MMA rate: per 64-deep k-block a CTA's smem serves the 12 MMAs' operand reads
-  // (128 + BN rows x 32 B each) plus the TMA fill of the next stage, ~128 B/clk in total.  Wider N tiles amortise the A rows,
-  // CTA pairs halve the B rows per CTA; rounds = ceil(units / resident CTAs or pairs) adds the wave quantisation and a fixed
-  // per-round cost covers pipeline fill + the last tile's exposed epilogue.
+  // N tile: BN = 128 halves the A-operand reads per output and the tile count; BN = 64 only where 128 would leave more than
+  // half of the SMs without a tile (rounds of resident CTAs, one CTA per SM)
   {
     const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
-    const int kblocks = taps * (src0.C / BK) + (src1 ? src1->C / BK : 0);
-    struct Cand { int bn; bool pair; double t_kb; };
-    // clocks per k-block from the sweep (zero operands, 1.9 GHz): single-CTA 64 / 128 run the DUAL form (two instructions per
-    // k-step), 256 the three-instruction form; pairs pay off only at BN = 256 (at BN = 128 they match the single-CTA pace on zeros
-    // and lose 14 % on real data under the power cap)
-    const Cand cands[] = {{64, false, 1000.0}, {128, false, g_dual_mode ? 1000.0 : 1100.0}, {256, false, 2060.0},
-                          {128, true, (g_pair_dual && g_terms == 3) ? g_pair_dual_tkb : g_pair_tkb[0]}, {256, true, g_pair_tkb[1]}};
-    double best = 1e300;
     L.BN = 64;
-    L.pair = false;
-    for (const Cand& c : cands) {
-      if (Cout % c.bn) continue;
-      if (g_force_bn && c.bn != g_force_bn && Cout % g_force_bn == 0) continue;   // tuning experiments only
-      const long long tiles = (long long)m_tiles * (Cout / c.bn);
-      if (c.pair && (g_pair_mode == 0 || w_batches != 1 || m_tiles % 2 != 0)) continue;
-      if (!c.pair && g_pair_mode == 1 && w_batches == 1 && m_tiles % 2 == 0 && c.bn >= 128) continue;   // forced pairs
-      const long long units = c.pair ? tiles / 2 : tiles;
-      const long long slots = c.pair ? num_sms / 2 : num_sms;
-      // PAIR + DUAL was only measured (and only pays) on layers with many tiles; smaller ones keep the single-CTA DUAL form
-      if (c.pair && c.bn == 128 && g_pair_dual && g_pair_mode != 1 && units < 2 * slots) continue;
-      const double rounds = (double)((units + slots - 1) / slots);
-      const double cost = rounds * (kblocks * c.t_kb + 1500.0);
-      if (cost < best) {
-        best = cost;
-        L.BN = c.bn;
-        L.pair = c.pair;
-      }
-    }
+    if (Cout % 128 == 0 && (long long)m_tiles * (Cout / 128) >= num_sms / 2) L.BN = 128;
+    if (g_force_bn && Cout % g_force_bn == 0) L.BN = g_force_bn;   // tests / tuning experiments only
   }
-  // pairs at BN = 128 run the PAIR + DUAL form when enabled (it needs the 3-term arithmetic), else the plain pair form
-  L.dual = g_dual_mode != 0 && L.BN <= 128 && (!L.pair || (L.BN == 128 && g_pair_dual && g_terms == 3));
   p.n_tiles = Cout / L.BN;
+  // CTA pairs (B tile multicast to two CTAs of a cluster) need an even number of M tiles and one weight matrix for all images.
+  // Not the default: on an H100 SXM at a 400 W limit the celeba forward (B = 16) took 80.5 ms with pairs on every layer of at least
+  // two waves of tiles and 74.6 ms without — the weight traffic they save is not what limits these layers.
+  {
+    const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
+    L.pair = g_pair_mode == 1 && w_batches == 1 && m_tiles % 2 == 0;
+  }
+  L.dual = g_dual_mode != 0 && (!L.pair || g_pair_dual != 0);
   p.mode0 = mode0;
   p.cb0 = src0.C / BK;
   p.kb0 = taps * p.cb0;
@@ -806,26 +606,18 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
   }
   p.Cout = Cout; p.ldc = out.ld; p.out = out.p;
   p.out_sx = out.ld; p.out_sy = (long long)out.W * out.ld; p.out_sn = (long long)out.H * out.W * out.ld;
-  DDNM_CHECK(out.C == Cout && out.ld % 8 == 0 && ((uintptr_t)out.p & 31) == 0, "output view misaligned (rows move as 32-byte vectors)");
+  DDNM_CHECK(out.C == Cout && out.ld % 2 == 0 && ((uintptr_t)out.p & 7) == 0, "output view misaligned (rows move as float2)");
   p.chanadd = chanadd; p.ca_ld = ca_ld; p.residual = residual; p.ldr = ldr; p.alpha = alpha; p.res_mode = res_mode;
   p.stats = out.st; p.st_ld = out.st_ld;
   p.terms = g_terms;
   if (out.st) DDNM_CHECK(p.bw * p.bh >= 32, "GroupNorm statistics need >= 32 pixels per image");
-  if (residual) DDNM_CHECK(ldr % 8 == 0 && ((uintptr_t)residual & 31) == 0, "residual misaligned (rows move as 32-byte vectors)");
-  // UMMA shared-memory descriptor, high word: SBO = 1024 B (8 rows x 128 B) >> 4 at bits [32,46), version = 1 at
-  // [46,48), layout SWIZZLE_128B (= 2) at [61,64).  (cute/arch/mma_sm100_desc.hpp SmemDescriptor)
-  p.desc_hi = g_desc_hi_override ? g_desc_hi_override : (64u | (1u << 14) | (2u << 29));
-  // Instruction descriptor: D = f32 (1 << 4), A = B = f16 (0), K-major both, N >> 3 at [17,23), M >> 4 at [24,29)
-  p.idesc = ((1u << 4) | ((uint32_t)(L.BN >> 3) << 17) | ((uint32_t)((L.pair ? 2 * BM : BM) >> 4) << 24)) ^ g_idesc_xor;
+  if (residual) DDNM_CHECK(ldr % 2 == 0 && ((uintptr_t)residual & 7) == 0, "residual misaligned (rows move as float2)");
+  if (chanadd) DDNM_CHECK(ca_ld % 2 == 0 && ((uintptr_t)chanadd & 7) == 0, "channel-add rows misaligned");
 
-  // halo-row form: pairs, 3x3 stride 1, tiles of 128 pixels of one row (W >= 128), fp32-grade arithmetic
-  L.halo = g_halo != 0 && L.pair && mode0 == TAPS_3X3 && p.bw == 128 && p.bh == 1 && p.bn == 1 && g_terms == 3 && p.b_batched == 0 &&
-           (L.BN == 256 || L.dual);
   const uint64_t ad[4] = {(uint64_t)src0.C, (uint64_t)src0.W, (uint64_t)src0.H, (uint64_t)src0.N};
   const uint32_t abox[4] = {(uint32_t)BK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
-  const uint32_t hbox[4] = {(uint32_t)BK, 130u, 1u, 1u};   // HALO: pixels x0-1 .. x0+128 of one row
-  L.a0h = make_map_f16(src0.hi, 4, ad, L.halo ? hbox : abox);
-  L.a0l = make_map_f16(src0.lo, 4, ad, L.halo ? hbox : abox);
+  L.a0h = make_map_f16(src0.hi, 4, ad, abox);
+  L.a0l = make_map_f16(src0.lo, 4, ad, abox);
   if (src1) {
     const uint64_t ad1[4] = {(uint64_t)src1->C, (uint64_t)src1->W, (uint64_t)src1->H, (uint64_t)src1->N};
     L.a1h = make_map_f16(src1->hi, 4, ad1, abox);
@@ -836,20 +628,14 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
   }
   const int Ktot = (p.kb0 + p.kb1) * BK;
   const uint64_t bd[3] = {(uint64_t)Ktot, (uint64_t)Cout, (uint64_t)w_batches};
-  const bool pd = L.pair && L.dual;
-  const uint32_t bbox[3] = {(uint32_t)BK, (uint32_t)(L.pair && !pd ? L.BN / 2 : L.BN), 1u};
+  const uint32_t bbox[3] = {(uint32_t)BK, (uint32_t)(L.pair ? L.BN / 2 : L.BN), 1u};   // PAIR: each CTA loads half of the B tile
   L.bh = make_map_f16(w_hi, 3, bd, bbox);
   L.bl = make_map_f16(w_lo, 3, bd, bbox);
-  L.b2 = L.bh;
-  if (pd) {
-    const uint32_t hbox[3] = {(uint32_t)BK, (uint32_t)(L.BN / 2), 1u};
-    L.b2 = make_map_f16(w_hi, 3, bd, hbox);
-  }
   const int total = p.tiles_x * p.tiles_y * p.tiles_n * p.n_tiles;
   L.grid = L.pair ? 2 * std::min(total / 2, num_sms / 2) : std::min(total, num_sms);
   // contiguous tile ranges per CTA where the GroupNorm sums of the output would otherwise be flushed at every tile: one N tile
   // (so consecutive tiles of a range share their channels) and several tiles per CTA
-  const int workers = L.pair ? L.grid / 2 : L.grid, units = L.pair ? total / 2 : total;
+  const int units = L.pair ? total / 2 : total, workers = L.pair ? L.grid / 2 : L.grid;
   p.deal = g_deal >= 0 ? g_deal : (out.st != nullptr && p.n_tiles == 1 && units >= 2 * workers ? 1 : 0);
   if (p.n_tiles != 1) p.deal = 0;
   L.flops = 2.0 * (double)out.pixels() * Cout * Ktot;
@@ -882,7 +668,7 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
   p.bw = 128; p.bh = 1; p.bn = 1;
   p.tiles_x = M / 128; p.tiles_y = heads; p.tiles_n = images;
   const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
-  // same sweep as the convolutions: BN = 128 beats 64 (fewer, larger instructions) unless it leaves most SMs idle
+  // as for the convolutions: BN = 128 unless it leaves most SMs idle
   L.BN = 64;
   if (N % 128 == 0 && (long long)m_tiles * (N / 128) >= num_sms / 2) L.BN = 128;
   L.dual = g_dual_mode != 0;
@@ -894,12 +680,10 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
   p.b_batched = 2;
   p.Cout = N; p.ldc = (int)out_sx; p.out = out;
   p.out_sn = out_sn; p.out_sy = out_sy; p.out_sx = out_sx;
-  DDNM_CHECK(out_sx % 8 == 0 && out_sy % 8 == 0 && out_sn % 8 == 0 && ((uintptr_t)out & 31) == 0, "attention GEMM output misaligned");
+  DDNM_CHECK(out_sx % 2 == 0 && out_sy % 2 == 0 && out_sn % 2 == 0 && ((uintptr_t)out & 7) == 0, "attention GEMM output misaligned");
   p.chanadd = nullptr; p.ca_ld = 0; p.residual = nullptr; p.ldr = 0; p.res_mode = 0; p.alpha = alpha;
   p.stats = nullptr; p.st_ld = 0;
   p.terms = g_terms;
-  p.desc_hi = g_desc_hi_override ? g_desc_hi_override : (64u | (1u << 14) | (2u << 29));
-  p.idesc = ((1u << 4) | ((uint32_t)(L.BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24)) ^ g_idesc_xor;
   const uint64_t ad[4] = {(uint64_t)K, (uint64_t)M, (uint64_t)heads, (uint64_t)images};
   const uint64_t as[3] = {(uint64_t)A.s_row, (uint64_t)A.s_head, (uint64_t)A.s_img};
   const uint32_t abox[4] = {(uint32_t)BK, 128u, 1u, 1u};
@@ -912,41 +696,85 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
   const uint32_t bbox[4] = {(uint32_t)BK, (uint32_t)L.BN, 1u, 1u};
   L.bh = make_map_f16(B.hi, 4, bd, bbox, bs);
   L.bl = make_map_f16(B.lo, 4, bd, bbox, bs);
-  L.b2 = L.bh;
   L.grid = std::min(m_tiles * p.n_tiles, num_sms);
   L.flops = 2.0 * (double)images * heads * M * (double)N * K;
   return L;
 }
 
-template <int BN, bool PAIR, bool DUAL, bool HALO = false>
+template <int BN, bool PAIR, bool DUAL, bool GN = false>
 static void launch_bn(const TcLaunch& L, cudaStream_t stream) {
-  using Cfg = TcCfg<BN, PAIR, DUAL, HALO>;
+  using Cfg = TcCfg<BN, DUAL>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set))
-    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_kernel<BN, PAIR, DUAL, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  launch_pdl(conv_tc_kernel<BN, PAIR, DUAL, HALO>, dim3(L.grid), dim3(HALO ? kTcThreads + 32 : kTcThreads), (size_t)Cfg::SMEM_BYTES, stream,
-             PAIR ? 2 : 1, L.a0h, L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.b2, L.p);
+    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_kernel<BN, PAIR, DUAL, GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+  launch_pdl(conv_tc_kernel<BN, PAIR, DUAL, GN>, dim3(L.grid), dim3(kTcThreads), (size_t)Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1, L.a0h,
+             L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.p, L.g);
   CUDA_CHECK(cudaGetLastError());
 }
 
+template <int BN>
+static void launch_forms(const TcLaunch& L, cudaStream_t stream) {
+  if (L.gn && L.dual) launch_bn<BN, false, true, true>(L, stream);
+  else if (L.gn) launch_bn<BN, false, false, true>(L, stream);
+  else if (L.pair && L.dual) launch_bn<BN, true, true>(L, stream);
+  else if (L.pair) launch_bn<BN, true, false>(L, stream);
+  else if (L.dual) launch_bn<BN, false, true>(L, stream);
+  else launch_bn<BN, false, false>(L, stream);
+}
+
+// ---- GN form: fused GroupNorm + SiLU + split + 3x3 convolution ----
+// Default OFF (env DDNM_GN_FUSED=1 / ddnm_tc_debug_gn_fused): per launch it saves the normalised planes' HBM round trip, but every
+// consumer warpgroup then waits for its own row loads before each k-block's MMAs.
+static int g_gn_enable = [] { const char* v = std::getenv("DDNM_GN_FUSED"); return v && *v ? std::atoi(v) : 0; }();
+void tc_debug_gn_fused(int on) { g_gn_enable = on; }
+
+static bool gn_shape_ok(const View& x, const View* side, int Cout, const View& out) {
+  if (out.W % 128 != 0 || x.C % BK != 0 || x.C > kGnMaxC || Cout % 64 != 0) return false;
+  if (x.H != out.H || x.W != out.W || x.N != out.N) return false;
+  if (x.ld % 4 != 0 || ((uintptr_t)x.p & 15) != 0) return false;
+  if (side && (side->C % BK != 0 || side->ld % 4 != 0 || ((uintptr_t)side->p & 15) != 0 || side->H != out.H || side->W != out.W ||
+               side->N != out.N))
+    return false;
+  return true;
+}
+
+bool tc_gn_eligible(const View& x, const View* side, int Cout, const View& out) { return g_gn_enable != 0 && gn_shape_ok(x, side, Cout, out); }
+
+TcLaunch tc_make_gn_launch(const View& x, const GnAffine& gn, const View* side, const __half* w_hi, const __half* w_lo, int Cout,
+                           const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int num_sms) {
+  DDNM_CHECK(gn_shape_ok(x, side, Cout, out), "fused GroupNorm convolution: unsupported shape");
+  DDNM_CHECK(g_terms == 3, "the fused GroupNorm convolution implements the fp32-grade (3-term) arithmetic only");
+  // the tiling, B operand and epilogue of a plain 3x3 launch over a placeholder A split of x's shape (its tensor maps are unused)
+  SplitView a;
+  a.hi = const_cast<__half*>(w_hi);
+  a.lo = const_cast<__half*>(w_lo);
+  a.N = x.N; a.H = x.H; a.W = x.W; a.C = x.C;
+  SplitView s1;
+  if (side) {
+    s1 = a;
+    s1.C = side->C;
+  }
+  const int gp = g_pair_mode;
+  g_pair_mode = 0;
+  TcLaunch L = tc_make_launch(a, TAPS_3X3, side ? &s1 : nullptr, w_hi, w_lo, 1, Cout, out, chanadd, ca_ld, residual, ldr, 1.0f, num_sms, 0);
+  g_pair_mode = gp;
+  L.gn = true;
+  L.dual = L.dual && L.BN == 64;   // GN + DUAL at BN = 128 exceeds the 168 registers per thread of three warpgroups (spills)
+  TcGnArgs& g = L.g;
+  g.x = x.p; g.x_ld = x.ld; g.C = x.C;
+  g.xs = side ? side->p : nullptr; g.xs_ld = side ? side->ld : 0;
+  g.norm = gn.gamma != nullptr ? 1 : 0;
+  if (g.norm) DDNM_CHECK(x.st != nullptr && x.C % gn.groups == 0, "normalisation needs the tensor's per-channel sums (View::st)");
+  g.st = x.st; g.st_ld = x.st_ld;
+  g.gamma = gn.gamma; g.beta = gn.beta; g.eps = gn.eps; g.groups = gn.groups; g.ss = gn.ss; g.ss_ld = gn.ss_ld; g.silu = gn.silu ? 1 : 0;
+  return L;
+}
+
 void tc_run(const TcLaunch& L, cudaStream_t stream) {
+  DDNM_CHECK(!L.pair || L.p.split_k == 1, "CTA pairs do not split K");
   switch (L.BN) {
-    case 256:
-      if (L.pair && L.halo) launch_bn<256, true, false, true>(L, stream);
-      else if (L.pair) launch_bn<256, true, false>(L, stream);
-      else launch_bn<256, false, false>(L, stream);
-      break;
-    case 128:
-      if (L.pair && L.dual && L.halo) launch_bn<128, true, true, true>(L, stream);
-      else if (L.pair && L.dual) launch_bn<128, true, true>(L, stream);
-      else if (L.pair) launch_bn<128, true, false>(L, stream);
-      else if (L.dual) launch_bn<128, false, true>(L, stream);
-      else launch_bn<128, false, false>(L, stream);
-      break;
-    case 64:
-      if (L.dual) launch_bn<64, false, true>(L, stream);
-      else launch_bn<64, false, false>(L, stream);
-      break;
+    case 128: launch_forms<128>(L, stream); break;
+    case 64: launch_forms<64>(L, stream); break;
     default: throw Error("bad BN");
   }
 }

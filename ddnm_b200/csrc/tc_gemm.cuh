@@ -1,5 +1,5 @@
-// tcgen05 implicit-GEMM convolution / GEMM with 3x fp16 split ("fp32-grade" products on the
-// 5th-gen tensor cores).  See tc_gemm.cu for the kernel; this header is the host-side launch record.
+// wgmma implicit-GEMM convolution / GEMM with 3x fp16 split ("fp32-grade" products on the
+// Hopper tensor cores).  See tc_gemm.cu for the kernel; this header is the host-side launch record.
 #pragma once
 #include "common.cuh"
 
@@ -36,20 +36,36 @@ struct TcParams {
   StatAcc* stats;              // optional GroupNorm sums of the OUTPUT: stats[(image*st_ld + co)*2 + {0,1}] += {sum, sumsq}
   int st_ld;
   int split_k = 1;             // > 1: this many CTAs per tile, each over its own k-block range, partial sums to out + ks * split_stride
-  long long split_stride = 0;  //      (single-CTA forms only; no chanadd / residual / stats: splitk_reduce applies them)
+  long long split_stride = 0;  //      (no chanadd / residual / stats: splitk_reduce applies them)
   int deal = 0;                // tile -> CTA map: 0 round-robin, 1 one contiguous range per CTA (see conv_tc_kernel)
   int terms;                   // 3: hi*hi + hi*lo + lo*hi (fp32-grade, default); 1: hi*hi only (plain fp16 inputs, fast mode)
-  uint32_t desc_hi;            // UMMA smem descriptor high word (SW128 K-major), see tc_gemm.cu
-  uint32_t idesc;              // UMMA instruction descriptor
+};
+
+// GN form (fused GroupNorm + SiLU + split + 3x3 convolution, see conv_tc_kernel): the A operand is produced from fp32 rows
+struct TcGnArgs {
+  const float* x = nullptr;       // fp32 NHWC source of the 3x3 taps, row pitch x_ld, C channels
+  int x_ld = 0, C = 0;
+  const float* xs = nullptr;      // optional fp32 NHWC raw input of the 1x1 shortcut (extra K blocks), row pitch xs_ld
+  int xs_ld = 0;
+  const StatAcc* st = nullptr;    // per-(image, channel) sums of x (View::st)
+  int st_ld = 0;
+  const float* gamma = nullptr;
+  const float* beta = nullptr;
+  float eps = 0.f;
+  int groups = 32;
+  const float* ss = nullptr;      // optional per-(image, channel) [scale(C) | shift(C)] rows (use_scale_shift_norm)
+  int ss_ld = 0;
+  int silu = 0, norm = 0;
 };
 
 struct TcLaunch {
-  CUtensorMap a0h, a0l, a1h, a1l, bh, bl, b2;   // b2: B_hi with a BN/2-row box (PAIR + DUAL form), else = bh
+  CUtensorMap a0h, a0l, a1h, a1l, bh, bl;   // PAIR: bh / bl have a BN/2-row box (each CTA of the pair loads half of the B tile)
   TcParams p;
   int BN = 128;
-  bool pair = false;           // CTA-pair kernel (cta_group::2, 256-row MMAs, cluster of 2)
-  bool halo = false;           // halo-row form: A staged once per (channel slice, dy) and shared by the three dx taps
-  bool dual = false;           // two partial accumulators per stage: hi*hi and hi*lo issued as one N = 2*BN instruction
+  bool pair = false;           // CTA-pair kernel (cluster of 2, B tile multicast to both CTAs)
+  bool dual = false;           // A_hi x [B_hi; B_lo] as one m64 x 2BN instruction, two partial accumulators
+  bool gn = false;             // GN form: A produced in the kernel from g
+  TcGnArgs g;
   int grid = 0;
   double flops = 0;            // algorithmic flops (2*M*N*K, counted once)
 };
@@ -77,7 +93,7 @@ struct GemmOperand {
 TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, int N, int K, int heads, int images, float* out,
                              long long out_sn, long long out_sy, long long out_sx, float alpha, int num_sms);
 
-// ---- fused GroupNorm + SiLU + split + 3x3 convolution (tc_gn_conv.cu): the A operand is produced inside the kernel ----
+// ---- fused GroupNorm + SiLU + split + 3x3 convolution (the GN form of conv_tc_kernel) ----
 struct GnAffine {
   const float* gamma = nullptr;   // nullptr: no normalisation (raw split)
   const float* beta = nullptr;
@@ -87,51 +103,19 @@ struct GnAffine {
   const float* ss = nullptr;      // optional per-(image, channel) [scale(C) | shift(C)] rows (use_scale_shift_norm, unet.py:250-252)
   int ss_ld = 0;
 };
-struct TcGnParams {
-  TcParams t;                     // tiling, B operand, epilogue (tile = 128 pixels of one row; pairs only)
-  const float* x;                 // fp32 NHWC source of the 3x3 taps, row pitch x_ld
-  int x_ld;
-  const float* xs;                // optional fp32 NHWC source of the 1x1 side input (nin_shortcut), row pitch xs_ld
-  int xs_ld;
-  const StatAcc* st_in;           // per-(image, channel) sums of x (View::st)
-  int st_ld_in;
-  const float* gamma;
-  const float* beta;
-  float eps;
-  int groups;
-  const float* ss;
-  int ss_ld;
-  int silu, norm;
-  int desc_mode;                  // 0: shifted start address only; 1: + base-offset field (descriptor bits [49,52))
-  int pf_dist;                    // L2 prefetch distance in units (0 = none)
-  long long* dbg;                 // optional (tests/diag): per-CTA clock counters, 16 per CTA — see conv_gn_tc_kernel
-};
-struct TcGnLaunch {
-  CUtensorMap bh, bl, b2;
-  TcGnParams g;
-  int BN = 128;
-  int grid = 0;
-  double flops = 0;
-};
 // x: fp32 activation with its GroupNorm sums; side: raw fp32 input of a 1x1 shortcut riding as extra K blocks (may be null);
 // w_hi/w_lo as for tc_make_launch with Ktot = 9*x.C + side.C.
 bool tc_gn_eligible(const View& x, const View* side, int Cout, const View& out);
-TcGnLaunch tc_make_gn_launch(const View& x, const GnAffine& gn, const View* side, const __half* w_hi, const __half* w_lo, int Cout,
-                             const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int num_sms);
-void tc_gn_run(const TcGnLaunch& L, cudaStream_t stream);
-void tc_debug_gn_desc_mode(int mode);   // tests: how the shifted A start address is described to the tensor core
-void tc_debug_gn_counters(long long* dev_buf);   // diag: where the fused kernel's warps spend their clocks (nullptr = off)
-void tc_debug_gn_pf_dist(int d);       // diag: L2 prefetch distance of fused launches built afterwards
-void tc_debug_gn_fused(int on);         // 1: eligible layers use the fused kernel; 0 (default): gn_apply + conv_tc
+TcLaunch tc_make_gn_launch(const View& x, const GnAffine& gn, const View* side, const __half* w_hi, const __half* w_lo, int Cout,
+                           const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int num_sms);
+void tc_debug_gn_fused(int on);      // 1: eligible layers of engines built afterwards use the GN form; 0 (default): gn_apply + conv_tc
 
-// debug knobs (tests only): override descriptor words for the NEXT launches built
-void tc_debug_override(uint32_t desc_hi, uint32_t idesc_xor);
-void tc_debug_force_bn(int bn);
-void tc_debug_halo(int on);         // 1 (default, env DDNM_HALO): eligible pair launches use the halo-row form
+// debug knobs (tests only): apply to the launches built afterwards
+void tc_debug_force_bn(int bn);      // 0 (default): heuristic, 64 / 128: force the N tile where Cout allows it
 void tc_debug_deal(int mode);        // -1 (default): contiguous tile ranges where they pay (one N tile + GroupNorm sums), 0 / 1: force
-void tc_debug_pair_dual(int on);     // 1 (default): CTA pairs at BN = 128 use the PAIR + DUAL form
-void tc_debug_dual_mode(int mode);   // 1: DUAL kernel for single-CTA BN <= 128 launches (default), 0: never
-void tc_debug_pair_mode(int mode);   // -1: cost model decides (default), 0: never, 1: CTA pairs wherever legal
+void tc_debug_pair_mode(int mode);   // -1 (default) / 0: no CTA pairs, 1: CTA pairs wherever legal
+void tc_debug_dual_mode(int mode);   // 1 (default): DUAL form for single-CTA launches, 0: never
+void tc_debug_pair_dual(int on);     // 1 (default): CTA pairs use the DUAL form too, 0: the plain pair form
 // number of fp16 product terms used by launches built from now on (3 = parity mode, 1 = fast mode)
 void tc_set_terms(int terms);
 int tc_get_terms();

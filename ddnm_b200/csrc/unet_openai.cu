@@ -28,7 +28,7 @@ void UNetOpenAI::emit_resblock(const std::string& p, const View& x, const View& 
   h.p = hbuf_; h.N = B_; h.H = out.H; h.W = out.W; h.C = Cout; h.ld = Cout;
   h.st = new_stats(Cout); h.st_ld = Cout;   // conv1's epilogue accumulates the sums out_layers.0 needs
   if (kind == RES_PLAIN && fused_ok(x, nullptr, Cout, h) && fused_ok(h, has_skip_conv ? &x : nullptr, Cout, out)) {
-    // wide maps: GroupNorm (+ scale-shift) + SiLU + fp16 split inside the convolution kernels (tc_gn_conv.cu)
+    // wide maps: GroupNorm (+ scale-shift) + SiLU + fp16 split inside the convolution kernel (conv_tc_kernel's GN form)
     TcWeights w1 = prep_weights(p + ".in_layers.2.weight", Cout, Cin, 9, "", 0);
     emit_tcgn(p + ".conv1", x, p + ".in_layers.0", nullptr, 0, nullptr, w1, Cout, h, P(p + ".in_layers.2.bias", Cout), 0, nullptr, 0);
     if (has_skip_conv) {

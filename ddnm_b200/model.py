@@ -5,7 +5,7 @@
     model.load_state_dict(state_dict)     # same keys/layout as the reference checkpoint
     et = model(xt, t)                     # same call as functions/svd_ddnm.py:47
 
-The forward pass runs entirely inside libddnm_b200.so (CUDA graph of hand-written sm_100a kernels); torch is
+The forward pass runs entirely inside libddnm_b200.so (CUDA graph of hand-written sm_90a kernels); torch is
 only used for tensor storage and the current stream.  Inference only (the reference samples under no_grad).
 """
 import ctypes as C

@@ -1,4 +1,4 @@
-/* ddnm_b200 — C ABI of the B200-native DDNM sampling engine (libddnm_b200.so).
+/* ddnm_b200 — C ABI of the H100-native DDNM sampling engine (libddnm_b200.so).
  *
  * The reference (wyhuai/DDNM) has no FFI: its hot path is reached through three Python call conventions
  * (SURVEY.md §8b).  Each entry point below names the reference interface it stands behind; the Python
@@ -229,39 +229,27 @@ int ddnm_conv_tc_bench(int N, int H, int W, int Cin, int Cout, int mode, int ite
 int ddnm_gnconv_chunk_bench(int N, int chunk, int H, int W, int Cin, int Cout, int iters, float* ms_per_pass);
 int ddnm_groupnorm(const float* x, int N, int H, int W, int C, int groups, const float* gamma, const float* beta, float eps,
                    int silu, float* out, void* stream);
-/* The fused form the engine uses for the wide layers (rows >= 128 pixels): out = conv3x3(silu?(groupnorm(x))) [+ conv1x1(side_x)] + bias
- * [+ residual] with the GroupNorm / SiLU / fp16 split applied INSIDE the convolution kernel (models.py:115-134 conv1 / conv2 +
- * nin_shortcut).  gamma == NULL: no normalisation.  iters > 0 additionally times `iters` launches into *ms_per_iter. */
+/* out = conv3x3(silu?(groupnorm(x))) [+ conv1x1(side_x)] + bias [+ residual] with the GroupNorm / SiLU / fp16 split applied INSIDE the
+ * convolution kernel (models.py:115-134 conv1 / conv2 + nin_shortcut), rows of >= 128 pixels.  gamma == NULL: no normalisation.
+ * iters > 0 additionally times `iters` launches into *ms_per_iter. */
 int ddnm_conv_gn_tc(const float* x, int N, int H, int W, int Cin, int groups, const float* gamma, const float* beta, float eps, int silu,
                     const float* w, const float* bias, int Cout, const float* side_x, int CinSide, const float* side_w,
                     const float* residual, float* out, int iters, float* ms_per_iter, void* stream);
-/* diag: device buffer of 16 int64 per CTA (>= 148 CTAs) that fused launches BUILT afterwards fill with clock counters — first warp
- * of transform group g at [5g..5g+4]: units, waiting for a free A slot, waiting for its register loads, converting + storing,
- * fence + arrive; UMMA issuer (leader CTAs): [10] total, [11] waiting for A units, [12] for B stages, [13] for a free accumulator */
-int ddnm_tc_debug_gn_counters(long long* dev_buf);
-/* diag: L2 prefetch distance (in A units) of fused launches built afterwards; 0 = none (default, env DDNM_GN_PF_DIST) */
-int ddnm_tc_debug_gn_pf_dist(int d);
-/* tests: 0 = shifted start address only, 1 = shifted start address + descriptor base-offset field */
-int ddnm_tc_debug_gn_desc_mode(int mode);
 /* 1: eligible layers (3x3, rows >= 128 pixels) of engines built afterwards run the fused GroupNorm convolution; 0 (default, also env
  * DDNM_GN_FUSED): gn_apply_kernel + conv_tc_kernel */
 int ddnm_tc_debug_gn_fused(int on);
-int ddnm_tc_debug_override(unsigned desc_hi, unsigned idesc_xor);
-/* tuning experiments: force the N-tile width of conv launches built afterwards (0 = heuristic) */
+/* tuning experiments: force the N-tile width (64 or 128) of conv launches built afterwards (0 = heuristic) */
 int ddnm_tc_debug_force_bn(int bn);
 /* tile -> CTA map of conv launches built afterwards: -1 (default) contiguous tile ranges per CTA on layers with one N tile that
  * produce GroupNorm sums, 0 round-robin everywhere, 1 contiguous wherever legal */
 int ddnm_tc_debug_deal(int mode);
-/* 1 (default, also env DDNM_HALO): CTA-pair 3x3 launches on rows >= 128 pixels stage the A operand once per (channel slice, row
- * offset) as a 130-pixel halo row shared by the three horizontal taps; 0: one TMA box per tap */
-int ddnm_tc_debug_halo(int on);
-/* 1 (default): CTA pairs at BN = 128 (Cout = 128 layers) use the PAIR + DUAL instruction form; 0: the plain pair form */
-int ddnm_tc_debug_pair_dual(int on);
-/* 1 (default): single-CTA launches with BN <= 128 issue hi*hi and hi*lo as one N = 2*BN instruction (two partial accumulators); 0: never */
-int ddnm_tc_debug_dual_mode(int mode);
-/* CTA-pair kernel (tcgen05 cta_group::2) for conv launches built afterwards: -1 (default) the cost model decides,
- * 0 never, 1 wherever legal */
+/* CTA pairs (cluster of 2 sharing the weight tile through TMA multicast) for conv launches built afterwards: -1 (default) and 0
+ * never (slower than single CTAs on the H100 networks), 1 wherever legal */
 int ddnm_tc_debug_pair_mode(int mode);
+/* 1 (default): single-CTA launches issue hi*hi and hi*lo as one m64 x 2BN instruction (two partial accumulators); 0: never */
+int ddnm_tc_debug_dual_mode(int mode);
+/* 1 (default): CTA pairs use that DUAL form as well; 0: the plain three-instruction pair form */
+int ddnm_tc_debug_pair_dual(int on);
 
 #ifdef __cplusplus
 }

@@ -11,7 +11,7 @@ GOLD = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu on the GPU box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu on a machine with one")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -28,7 +28,7 @@ def pytest_collection_modifyitems(config, items):
 @pytest.fixture(scope="session", autouse=True)
 def built_library():
     """The tests exercise the in-tree libddnm_b200.so; compile it first if this checkout has not been built yet
-    (nvcc cross-compiles sm_100a without a GPU).  On the GPU box the prebuilt library travels with the snapshot."""
+    (nvcc cross-compiles sm_90a without a GPU)."""
     from ddnm_b200 import _lib
     if not os.path.exists(_lib.LIB_PATH):
         import shutil
@@ -38,7 +38,16 @@ def built_library():
     return _lib.LIB_PATH
 
 
+def _golden(name):
+    """tests/golden/<name>.npz merged with its <name>.part<i>.npz continuation files (fixtures are split to stay under 1 MB)."""
+    import glob
+    import numpy as np
+    arrays = dict(np.load(os.path.join(GOLD, name + ".npz")))
+    for part in sorted(glob.glob(os.path.join(GOLD, name + ".part*.npz"))):
+        arrays.update(np.load(part))
+    return arrays
+
+
 @pytest.fixture(scope="session")
 def gold():
-    import numpy as np
-    return {name: np.load(os.path.join(GOLD, name + ".npz")) for name in ("unet_simple", "unet_openai", "operators", "sampler_tiny", "simplified", "general_a", "runner_io", "guided_tiny", "fullsize", "sr16", "simplified_r2", "hq")}
+    return {name: _golden(name) for name in ("unet_simple", "unet_openai", "operators", "sampler_tiny", "simplified", "general_a", "runner_io", "guided_tiny", "fullsize", "sr16", "simplified_r2", "hq")}
