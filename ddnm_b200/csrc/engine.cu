@@ -172,6 +172,7 @@ void UNetEngine::emit_tc(const std::string& name, const SplitView& a, int mode, 
     DDNM_CHECK(!Ls.pair && Ls.BN == L.BN, "split-K: tile shape changed");
     Ls.p.split_k = S;
     Ls.p.split_stride = stride;
+    Ls.halo = false;   // k-block ranges of a split need not be whole A units
     Ls.grid = std::min(tiles * S, num_sms_);
     add_op(name, "tc", L.flops, bytes, [Ls](cudaStream_t s) { tc_run(Ls, s); });
     add_op(name + ".splitk_reduce", "reduce", 0, (double)(S + 1 + (residual ? 1 : 0)) * stride * 4,

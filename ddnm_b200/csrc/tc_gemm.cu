@@ -24,6 +24,15 @@
 //         the B tile, multicast into both CTAs' shared memory, so every weight row crosses L2 -> SM once per pair instead of twice.
 //         A stage may be refilled only when the consumers of BOTH CTAs have released it: each empty barrier counts the arrivals of
 //         the 16 consumer warps of the cluster.
+//   HALO: 3x3 stride-1 and upsample-phase (2x2) launches whose tile rows are 64-pixel runs of image rows (bw % 64 == 0, one image
+//         per tile).  The three column taps dx of a (dy, 64-channel slice) read the same image rows shifted by one pixel, so the
+//         producer loads them once, as a halo unit of (bw + 2) x bh pixels (bw + 1 for the upsample phases) in hi + lo, and the
+//         K order becomes (dy, slice, dx).  Each dx k-block reads the unit through a descriptor whose start is shifted by 128 B
+//         per pixel; wgmma applies the 128B swizzle to absolute shared-memory address bits, as TMA does when it writes the
+//         1024 B-aligned unit, so the shifted start needs no base offset (the same rule that lets the K advance add 32 B).  The
+//         A units have a ring of their own (HALO_UNITS, own full / empty barriers) next to a ring of 4 B stages; a unit goes back to
+//         the producer once the wgmma group of its last dx k-block has completed.  Launches with a 1x1 side input keep the per-tap
+//         form (see tc_make_launch).
 // And one with another A operand:
 //   GN:   fused GroupNorm + SiLU + fp16 split + 3x3 convolution (+ 1x1 shortcut as extra K blocks) on rows of >= 128 pixels.  Each
 //         consumer warpgroup reads its 64 pixels of the shifted fp32 rows itself, applies the per-(image, channel) affine of the
@@ -43,12 +52,21 @@ static constexpr int BK = 64;                      // fp16 elements = 128 bytes 
 static constexpr int A_PLANE_BYTES = BM * BK * 2;  // 16 KiB
 static constexpr int kGnMaxC = 512;                // GN form: widest normalised input
 
-template <int BN, bool DUAL>
+// HALO form: one A plane of a unit holds the halo rows of a tile, (bw + 2) x bh pixels of 128 B (at most 132 rows), 1024 B-aligned.
+// 2 units + 4 B stages: one unit feeds 3 (2) k-blocks, so the A ring still runs as far ahead as the B ring; celeba forward (B = 16,
+// CUDA graph) on an H100 SXM at 700 W: 58.2 ms, against 58.9 with 3 units + 3 B stages and 61.4 for the per-tap form.
+static constexpr int HALO_PLANE_BYTES = 17 * 1024;
+static constexpr int HALO_UNITS = 2;
+
+template <int BN, bool DUAL, bool HALO = false>
 struct TcCfg {
   static constexpr int B_PLANE_BYTES = BN * BK * 2;
-  static constexpr int STAGE_BYTES = 2 * A_PLANE_BYTES + 2 * B_PLANE_BYTES;   // A_hi, A_lo, B_hi, B_lo
-  static constexpr int STAGES = BN == 64 ? 4 : 3;
-  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  // without HALO one stage is {A_hi, A_lo, B_hi, B_lo}; with HALO the A units have their own ring in front of the B stages
+  static constexpr int A_UNIT_BYTES = 2 * HALO_PLANE_BYTES;
+  static constexpr int A_RING_BYTES = HALO ? HALO_UNITS * A_UNIT_BYTES : 0;
+  static constexpr int STAGE_BYTES = (HALO ? 0 : 2 * A_PLANE_BYTES) + 2 * B_PLANE_BYTES;
+  static constexpr int STAGES = (HALO || BN == 64) ? 4 : 3;
+  static constexpr int RING_BYTES = A_RING_BYTES + STAGES * STAGE_BYTES;
   // GroupNorm sums of a tile: per-warp column partials (8 warps x BN x {sum, sumsq}) and the running (value, compensation) pairs
   // of up to 4 images per tile x {sum, sumsq} x BN columns
   static constexpr int PART_BYTES = 8 * BN * 8;
@@ -85,20 +103,26 @@ __device__ __forceinline__ void gn_store_row(uint8_t* a_hi, int row, int chunk0,
   }
 }
 
-template <int BN, bool PAIR, bool DUAL, bool GN>
+template <int BN, bool PAIR, bool DUAL, bool GN, bool HALO>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant__ CUtensorMap tm_a0l,
                const __grid_constant__ CUtensorMap tm_a1h, const __grid_constant__ CUtensorMap tm_a1l,
                const __grid_constant__ CUtensorMap tm_bh, const __grid_constant__ CUtensorMap tm_bl, const TcParams p,
                const TcGnArgs g) {
   static_assert(!GN || !PAIR, "the GN form runs on single CTAs");
-  using Cfg = TcCfg<BN, DUAL>;
+  static_assert(!HALO || (!PAIR && !GN), "the HALO form runs on single CTAs with TMA-loaded A");
+  using Cfg = TcCfg<BN, DUAL, HALO>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + Cfg::RING_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  auto a_full_bar = [&](int u) { return bar_base + 8u * (2 * STAGES + u); };                // HALO: A units
+  auto a_empty_bar = [&](int u) { return bar_base + 8u * (2 * STAGES + HALO_UNITS + u); };
+  // HALO: k-blocks per A unit of the source-0 taps (the dx taps of one dy) and the unit's pixels per row
+  const int halo_r = p.mode0 == TAPS_UP2X2 ? 2 : 3;
+  const int halo_w = p.bw + halo_r - 1;
   uint8_t* stat_smem = smem_raw + (bar_base + 256u - smem_u32(smem_raw));
   float2* part = reinterpret_cast<float2*>(stat_smem);                    // [warp][BN] {sum, sumsq} over the warp's 16 rows
   float2* run = reinterpret_cast<float2*>(stat_smem + Cfg::PART_BYTES);   // [image slot][which][BN] {value, compensation}
@@ -151,6 +175,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
       mbar_init(full_bar(s), 1);    // the producer's expect_tx arrive
       mbar_init(empty_bar(s), PAIR ? 16 : 8);   // one arrive per consumer warp (of both CTAs of a pair)
     }
+    if (HALO) {
+      for (int u = 0; u < HALO_UNITS; ++u) {
+        mbar_init(a_full_bar(u), 1);
+        mbar_init(a_empty_bar(u), 8);
+      }
+    }
     mbar_fence_init();
   }
   if (PAIR) cluster_sync_all();   // the peer's barriers exist before any multicast or remote arrive can reach them
@@ -172,21 +202,45 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
     // ------------------------------------------------ TMA producer ------------------------------------------------
     if (lane == 0) {
       uint32_t stage = 0, phase = 0;
+      uint32_t aunit = 0, aphase = 0;   // HALO: A ring position
       const bool lo = p.terms != 1;
-      // GN: only the B planes arrive by TMA (the consumers write A themselves)
-      const uint32_t stage_tx = GN ? 2u * Cfg::B_PLANE_BYTES : (uint32_t)(lo ? Cfg::STAGE_BYTES : Cfg::STAGE_BYTES / 2);
+      const uint32_t planes = lo ? 2u : 1u;
+      // GN / HALO: only the B planes arrive with a stage (GN: the consumers write A themselves)
+      const uint32_t stage_tx = (GN || HALO) ? planes * Cfg::B_PLANE_BYTES : (uint32_t)(lo ? Cfg::STAGE_BYTES : Cfg::STAGE_BYTES / 2);
       for (int u = unit_begin; u < unit_end; u += unit_step) {
         int n_idx, x0, y0, n0;
         decode(tile_of(u), n_idx, x0, y0, n0);
         const int bz = p.b_batched == 1 ? n0 : 0;
         const int kb_lo = k_lo(u), kb_hi = k_hi(u);
         for (int kb = kb_lo; kb < kb_hi; ++kb) {
+          int bkb = kb;   // the weights' k-block (tap-major, see tc_make_launch)
+          if constexpr (HALO) {
+            // k order (dy, slice, dx); a new A unit at dx == 0
+            const int ua = kb / halo_r, dx = kb - ua * halo_r, dy = ua / p.cb0, cs = ua - dy * p.cb0;
+            bkb = (dy * halo_r + dx) * p.cb0 + cs;
+            if (dx == 0) {
+              mbar_wait(a_empty_bar(aunit), aphase ^ 1u);
+              const uint32_t ua_s = smem_base + aunit * Cfg::A_UNIT_BYTES;
+              const uint32_t fa = a_full_bar(aunit);
+              // halo rows y0 + dy - 1 (+ the phase row), columns from x0 - 1 (+ the phase column); borders are TMA zero fill
+              const int cy = y0 + dy - 1 + p.up_py, cx = x0 - 1 + p.up_px;
+              mbar_expect_tx(fa, planes * (uint32_t)(halo_w * p.bh * 128));
+              tma_load_4d(ua_s, &tm_a0h, fa, cs * BK, cx, cy, n0);
+              if (lo) tma_load_4d(ua_s + HALO_PLANE_BYTES, &tm_a0l, fa, cs * BK, cx, cy, n0);
+            }
+            if (dx == halo_r - 1) {
+              if (++aunit == HALO_UNITS) {
+                aunit = 0;
+                aphase ^= 1u;
+              }
+            }
+          }
           mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint32_t sb = sa + 2 * A_PLANE_BYTES;
+          const uint32_t sa = smem_base + Cfg::A_RING_BYTES + stage * Cfg::STAGE_BYTES;
+          const uint32_t sb = HALO ? sa : sa + 2 * A_PLANE_BYTES;
           const uint32_t fb = full_bar(stage);
           mbar_expect_tx(fb, stage_tx);
-          if (GN) {
+          if (GN || HALO) {
           } else if (kb < p.kb0) {
             const int tap = kb / p.cb0;
             const int c = (kb - tap * p.cb0) * BK;
@@ -220,8 +274,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
             tma_load_4d(sb, &tm_bh, fb, kb * BK, n_idx * BN, y0, n0);
             if (lo) tma_load_4d(sb + Cfg::B_PLANE_BYTES, &tm_bl, fb, kb * BK, n_idx * BN, y0, n0);
           } else {
-            tma_load_3d(sb, &tm_bh, fb, kb * BK, n_idx * BN, bz);
-            if (lo) tma_load_3d(sb + Cfg::B_PLANE_BYTES, &tm_bl, fb, kb * BK, n_idx * BN, bz);
+            tma_load_3d(sb, &tm_bh, fb, bkb * BK, n_idx * BN, bz);
+            if (lo) tma_load_3d(sb + Cfg::B_PLANE_BYTES, &tm_bl, fb, bkb * BK, n_idx * BN, bz);
           }
           if (++stage == STAGES) {
             stage = 0;
@@ -236,12 +290,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
   // columns 8j + 2(lane % 4) + {0, 1} of rows r0 = 16 warp + lane / 4 (d[4j], d[4j+1]) and r0 + 8 (d[4j+2], d[4j+3])
   const int wg = warp >> 2;
   const uint32_t a_row_off = (uint32_t)wg * 64u * 128u;
+  // HALO: the warpgroup's first pixel (yi, xi) inside the tile, as a row of the halo unit
+  const uint32_t halo_row_off = (uint32_t)(((wg * 64) / p.bw) * halo_w + (wg * 64) % p.bw) * 128u;
   const int r0 = warp * 16 + (lane >> 2);
   const int cq = (lane & 3) * 2;
   const int tid = threadIdx.x;
   const int ppi = p.bw * p.bh;                // pixels (tile rows) per image
   const int wpi = ppi >= 128 ? 8 : ppi / 16;  // warps per image slot of the tile
   uint32_t stage = 0, phase = 0;
+  uint32_t a_done = 0;   // HALO: A units consumed by this CTA's earlier tiles (ring slot = count % HALO_UNITS, parity = count / HALO_UNITS)
   if (p.stats) {
     for (int i = tid; i < 4 * 2 * BN; i += kConsumerThreads) run[i] = make_float2(0.f, 0.f);
   }
@@ -253,6 +310,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
       mbar_arrive(empty_bar(s));
       if (PAIR) mbar_arrive_cluster(empty_bar(s), rank ^ 1u);
     }
+  };
+  auto release_a = [&](int a) {
+    if (lane == 0) mbar_arrive(a_empty_bar(a));
   };
   for (int u = unit_begin; u < unit_end; u += unit_step) {
     const int kb_lo = k_lo(u), kb_hi = k_hi(u);
@@ -291,8 +351,28 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
       }
     }
     for (int kb = kb_lo; kb < kb_hi; ++kb) {
+      uint32_t a_base = smem_base + stage * Cfg::STAGE_BYTES + a_row_off;   // this warpgroup's rows of the A_hi plane
+      uint32_t a_plane = A_PLANE_BYTES;                                     // A_hi -> A_lo
+      uint32_t a_unit = 0;                                                  // HALO: this k-block's A unit, counted over the CTA's tiles
+      bool a_first = false;                                                 //       and whether the k-block is the unit's first reader
+      if constexpr (HALO) {
+        // derived from kb instead of carried across iterations: at BN = 128 with DUAL the accumulator leaves no spare registers
+        // HALO launches have no side input, so kb < p.kb0 always holds.  The guard and the select below only steer ptxas: written
+        // without them, the BN = 128 DUAL instantiation spills 60 / 96 B (stores / loads) instead of 40 / 76
+        int ua = 0, dx = 0;
+        if (kb < p.kb0) {
+          ua = halo_r == 3 ? (int)(__umulhi((uint32_t)kb, 0xAAAAAAABu) >> 1) : kb >> 1;
+          dx = kb - ua * halo_r;
+        }
+        a_unit = a_done + (uint32_t)ua;
+        a_first = dx == 0;
+        if (a_first) mbar_wait(a_full_bar(a_unit % HALO_UNITS), (a_unit / HALO_UNITS) & 1u);
+        a_base = smem_base + (a_unit % HALO_UNITS) * Cfg::A_UNIT_BYTES + (kb < p.kb0 ? halo_row_off + 128u * dx : a_row_off);
+        a_plane = HALO_PLANE_BYTES;
+      }
       mbar_wait(full_bar(stage), phase);
-      const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
+      const uint32_t sa = smem_base + Cfg::A_RING_BYTES + stage * Cfg::STAGE_BYTES;
+      const uint32_t sb = HALO ? sa : sa + 2 * A_PLANE_BYTES;
       if constexpr (GN) {
         // this warpgroup's 64 A rows: pixel x0 + row of row y0 (tiles are 128 pixels of one row), shifted by the tap
         const int rr = (tid & 127) >> 1, half = tid & 1, row = wg * 64 + rr;
@@ -335,10 +415,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to wgmma
         named_bar_sync(2 + wg, 128);
       }
-      const uint64_t ah = wgmma_desc_sw128(sa + a_row_off);
-      const uint64_t al = wgmma_desc_sw128(sa + A_PLANE_BYTES + a_row_off);
-      const uint64_t bh = wgmma_desc_sw128(sa + 2 * A_PLANE_BYTES);
-      const uint64_t bl = wgmma_desc_sw128(sa + 2 * A_PLANE_BYTES + Cfg::B_PLANE_BYTES);
+      const uint64_t ah = wgmma_desc_sw128(a_base);
+      const uint64_t al = wgmma_desc_sw128(a_base + a_plane);
+      const uint64_t bh = wgmma_desc_sw128(sb);
+      const uint64_t bl = wgmma_desc_sw128(sb + Cfg::B_PLANE_BYTES);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k) {
@@ -364,9 +444,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
         stage = 0;
         phase ^= 1u;
       }
+      // and so has the previous A unit if that k-block was its last reader (this one opens a new unit)
+      if (HALO && a_first && kb != kb_lo) release_a((a_unit - 1) % HALO_UNITS);
     }
     wgmma_wait<0>();
     if (prev >= 0) release(prev);
+    if constexpr (HALO) {
+      a_done += p.cb0 * halo_r;   // the tile's units
+      release_a((a_done - 1) % HALO_UNITS);
+    }
 
     // ---- epilogue: rows r0 and r0 + 8 of this tile, 2 adjacent columns per 8-column group ----
     int n_idx, x0, y0, n0;
@@ -548,6 +634,9 @@ static int g_dual_mode = 1;    // 1: single-CTA launches use the DUAL form (defa
 void tc_debug_dual_mode(int mode) { g_dual_mode = mode; }
 static int g_pair_dual = 1;    // 1: CTA pairs use the DUAL form as well (default), 0: the plain three-instruction pair form
 void tc_debug_pair_dual(int on) { g_pair_dual = on; }
+// HALO form wherever legal (see tc_make_launch); env DDNM_HALO=0 / tc_debug_halo(0) keep every launch on one A load per k-block
+static int g_halo_enable = [] { const char* v = std::getenv("DDNM_HALO"); return v && *v ? std::atoi(v) : 1; }();
+void tc_debug_halo(int on) { g_halo_enable = on; }
 static int g_deal = -1;
 void tc_debug_deal(int mode) {
   DDNM_CHECK(mode >= -1 && mode <= 1, "deal mode must be -1 (default rule), 0 (round-robin) or 1 (contiguous ranges)");
@@ -618,6 +707,16 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
   const uint32_t abox[4] = {(uint32_t)BK, (uint32_t)p.bw, (uint32_t)p.bh, (uint32_t)p.bn};
   L.a0h = make_map_f16(src0.hi, 4, ad, abox);
   L.a0l = make_map_f16(src0.lo, 4, ad, abox);
+  // HALO form: stride-1 taps on tiles whose warpgroups each own 64 consecutive pixels of one image row (one image per tile).  The
+  // halo maps are kept next to the plain ones: a launch that is later split along K (UNetEngine::emit_tc) runs without them.
+  // Not with a 1x1 side input: its k-blocks have no taps to share, and as one A unit each they left the celeba conv2 + shortcut
+  // launches at 128^2 / 256^2 up to 12 % slower than the per-tap form (whole forward: 60.1 ms with them in the HALO form, 58.2 without).
+  L.halo = g_halo_enable != 0 && !L.pair && (mode0 == TAPS_3X3 || mode0 == TAPS_UP2X2) && p.bw % 64 == 0 && p.bn == 1 && !src1;
+  if (L.halo) {
+    const uint32_t hbox[4] = {(uint32_t)BK, (uint32_t)(p.bw + (mode0 == TAPS_UP2X2 ? 1 : 2)), (uint32_t)p.bh, 1u};
+    L.hh = make_map_f16(src0.hi, 4, ad, hbox);
+    L.hl = make_map_f16(src0.lo, 4, ad, hbox);
+  }
   if (src1) {
     const uint64_t ad1[4] = {(uint64_t)src1->C, (uint64_t)src1->W, (uint64_t)src1->H, (uint64_t)src1->N};
     L.a1h = make_map_f16(src1->hi, 4, ad1, abox);
@@ -701,20 +800,22 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
   return L;
 }
 
-template <int BN, bool PAIR, bool DUAL, bool GN = false>
+template <int BN, bool PAIR, bool DUAL, bool GN = false, bool HALO = false>
 static void launch_bn(const TcLaunch& L, cudaStream_t stream) {
-  using Cfg = TcCfg<BN, DUAL>;
+  using Cfg = TcCfg<BN, DUAL, HALO>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set))
-    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_kernel<BN, PAIR, DUAL, GN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  launch_pdl(conv_tc_kernel<BN, PAIR, DUAL, GN>, dim3(L.grid), dim3(kTcThreads), (size_t)Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1, L.a0h,
-             L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.p, L.g);
+    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_kernel<BN, PAIR, DUAL, GN, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+  launch_pdl(conv_tc_kernel<BN, PAIR, DUAL, GN, HALO>, dim3(L.grid), dim3(kTcThreads), (size_t)Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1,
+             HALO ? L.hh : L.a0h, HALO ? L.hl : L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.p, L.g);
   CUDA_CHECK(cudaGetLastError());
 }
 
 template <int BN>
 static void launch_forms(const TcLaunch& L, cudaStream_t stream) {
-  if (L.gn && L.dual) launch_bn<BN, false, true, true>(L, stream);
+  if (L.halo && L.dual) launch_bn<BN, false, true, false, true>(L, stream);
+  else if (L.halo) launch_bn<BN, false, false, false, true>(L, stream);
+  else if (L.gn && L.dual) launch_bn<BN, false, true, true>(L, stream);
   else if (L.gn) launch_bn<BN, false, false, true>(L, stream);
   else if (L.pair && L.dual) launch_bn<BN, true, true>(L, stream);
   else if (L.pair) launch_bn<BN, true, false>(L, stream);
@@ -759,6 +860,7 @@ TcLaunch tc_make_gn_launch(const View& x, const GnAffine& gn, const View* side, 
   TcLaunch L = tc_make_launch(a, TAPS_3X3, side ? &s1 : nullptr, w_hi, w_lo, 1, Cout, out, chanadd, ca_ld, residual, ldr, 1.0f, num_sms, 0);
   g_pair_mode = gp;
   L.gn = true;
+  L.halo = false;
   L.dual = L.dual && L.BN == 64;   // GN + DUAL at BN = 128 exceeds the 168 registers per thread of three warpgroups (spills)
   TcGnArgs& g = L.g;
   g.x = x.p; g.x_ld = x.ld; g.C = x.C;
@@ -772,6 +874,8 @@ TcLaunch tc_make_gn_launch(const View& x, const GnAffine& gn, const View* side, 
 
 void tc_run(const TcLaunch& L, cudaStream_t stream) {
   DDNM_CHECK(!L.pair || L.p.split_k == 1, "CTA pairs do not split K");
+  DDNM_CHECK(!L.halo || (L.p.split_k == 1 && !L.pair && !L.gn && L.p.kb1 == 0),
+             "the HALO form runs unsplit single-CTA launches with TMA-loaded A and no 1x1 side input");
   switch (L.BN) {
     case 128: launch_forms<128>(L, stream); break;
     case 64: launch_forms<64>(L, stream); break;

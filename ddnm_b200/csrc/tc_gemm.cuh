@@ -60,11 +60,13 @@ struct TcGnArgs {
 
 struct TcLaunch {
   CUtensorMap a0h, a0l, a1h, a1l, bh, bl;   // PAIR: bh / bl have a BN/2-row box (each CTA of the pair loads half of the B tile)
+  CUtensorMap hh, hl;          // HALO: source 0 with a halo-row box {64, bw + 2 (up2: bw + 1), bh, 1}
   TcParams p;
   int BN = 128;
   bool pair = false;           // CTA-pair kernel (cluster of 2, B tile multicast to both CTAs)
   bool dual = false;           // A_hi x [B_hi; B_lo] as one m64 x 2BN instruction, two partial accumulators
   bool gn = false;             // GN form: A produced in the kernel from g
+  bool halo = false;           // HALO form: one A load per (dy, channel slice) feeds the dx taps; needs split_k == 1
   TcGnArgs g;
   int grid = 0;
   double flops = 0;            // algorithmic flops (2*M*N*K, counted once)
@@ -116,6 +118,7 @@ void tc_debug_deal(int mode);        // -1 (default): contiguous tile ranges whe
 void tc_debug_pair_mode(int mode);   // -1 (default) / 0: no CTA pairs, 1: CTA pairs wherever legal
 void tc_debug_dual_mode(int mode);   // 1 (default): DUAL form for single-CTA launches, 0: never
 void tc_debug_pair_dual(int on);     // 1 (default): CTA pairs use the DUAL form too, 0: the plain pair form
+void tc_debug_halo(int on);          // 1 (default, env DDNM_HALO): HALO form wherever legal, 0: never
 // number of fp16 product terms used by launches built from now on (3 = parity mode, 1 = fast mode)
 void tc_set_terms(int terms);
 int tc_get_terms();

@@ -250,6 +250,10 @@ int ddnm_tc_debug_pair_mode(int mode);
 int ddnm_tc_debug_dual_mode(int mode);
 /* 1 (default): CTA pairs use that DUAL form as well; 0: the plain three-instruction pair form */
 int ddnm_tc_debug_pair_dual(int on);
+/* 1 (default, also env DDNM_HALO): 3x3 stride-1 and upsample-phase conv launches built afterwards on maps >= 64 px wide and without
+ * a 1x1 side input load each
+ * (dy, 64-channel slice) of the activation once as halo rows for all column taps; 0: one A load per tap */
+int ddnm_tc_debug_halo(int on);
 
 #ifdef __cplusplus
 }
