@@ -442,6 +442,11 @@ int ddnm_tc_debug_halo(int on) {
   tc_debug_halo(on);
   DDNM_API_END
 }
+int ddnm_tc_debug_pingpong(int on) {
+  DDNM_API_BEGIN
+  tc_debug_pingpong(on);
+  DDNM_API_END
+}
 int ddnm_tc_debug_force_bn(int bn) {
   DDNM_API_BEGIN
   tc_debug_force_bn(bn);

@@ -264,6 +264,11 @@ __device__ __forceinline__ void tma_load_3d_multicast(uint32_t dst, const void* 
       : "memory");
 }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+// warpgroup-wide register reallocation (warp-specialised kernels): every thread of the warpgroup executes the same instruction
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // acc += p, independent of the order of concurrent adds.  p is converted (exactly, unless it has bits below 2^-48) to a signed
 // fixed-point integer X with 48 fractional bits, and X = W1 * 2^32 + W0 (W0 = X mod 2^32 >= 0, W1 = floor(X / 2^32)) is added

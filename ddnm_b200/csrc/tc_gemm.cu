@@ -39,6 +39,8 @@
 //         normalisation (from the producer-side GroupNorm sums, plus scale-shift), SiLU, splits to fp16 hi / lo and stores them in
 //         the 128B-swizzled K-major layout TMA would have written; `fence.proxy.async` makes the generic-proxy stores visible to
 //         its wgmma.  The producer loads only the weights.  The fp16 planes of the activation never exist in HBM.
+// conv_tc_pingpong_kernel (below) runs the single-CTA launches without GN where CTAs walk several tiles: each consumer warpgroup
+// owns a whole tile, and the two take turns on the tensor cores so one tile's epilogue overlaps the next tile's MMAs.
 #include "tc_gemm.cuh"
 
 #include <cstdlib>
@@ -103,6 +105,220 @@ __device__ __forceinline__ void gn_store_row(uint8_t* a_hi, int row, int chunk0,
   }
 }
 
+// output tile -> (N tile, first column, first row, first image of the M tile)
+__device__ __forceinline__ void tc_decode(const TcParams& p, int tile, int& n_idx, int& x0, int& y0, int& n0) {
+  n_idx = tile % p.n_tiles;
+  const int m = tile / p.n_tiles;
+  const int tx = m % p.tiles_x;
+  const int t2 = m / p.tiles_x;
+  const int ty = t2 % p.tiles_y;
+  const int tn = t2 / p.tiles_y;
+  x0 = tx * p.bw;
+  y0 = ty * p.bh;
+  n0 = tn * p.bn;
+}
+
+// Barriers behind the ring: full / empty per B stage, then (HALO) full / empty per A unit, then the ping-pong kernel's MMA turns
+template <int STAGES>
+struct TcBars {
+  uint32_t base;
+  __device__ uint32_t full(int s) const { return base + 8u * s; }
+  __device__ uint32_t empty(int s) const { return base + 8u * (STAGES + s); }
+  __device__ uint32_t a_full(int u) const { return base + 8u * (2 * STAGES + u); }
+  __device__ uint32_t a_empty(int u) const { return base + 8u * (2 * STAGES + HALO_UNITS + u); }
+  __device__ uint32_t turn(int w) const { return base + 8u * (2 * STAGES + 2 * HALO_UNITS + w); }
+};
+
+// The TMA producer's position in the B-stage ring and (HALO) in the A-unit ring
+struct TcRing {
+  uint32_t stage = 0, phase = 0;
+  uint32_t aunit = 0, aphase = 0;
+};
+
+// TMA loads of the k-blocks [kb_lo, kb_hi) of one output tile, issued by one thread: per k-block the B planes into the next stage
+// and the A operand — the tap-shifted window (3x3, stride-2 phase, upsample phase), the 1x1 side input, or (HALO) one halo unit
+// per (dy, channel slice) at its first dx k-block.  GN: only the B planes (the consumers write A).  PAIR: this CTA's half of the B
+// tile, multicast into both CTAs of the pair.
+template <class Cfg, bool PAIR, bool GN, bool HALO>
+__device__ __forceinline__ void tc_produce_tile(const CUtensorMap* tm_a0h, const CUtensorMap* tm_a0l, const CUtensorMap* tm_a1h,
+                                                const CUtensorMap* tm_a1l, const CUtensorMap* tm_bh, const CUtensorMap* tm_bl,
+                                                const TcParams& p, uint32_t smem_base, TcBars<Cfg::STAGES> bars, int tile, int kb_lo,
+                                                int kb_hi, uint32_t rank, TcRing& r) {
+  const int halo_r = p.mode0 == TAPS_UP2X2 ? 2 : 3;
+  const int halo_w = p.bw + halo_r - 1;
+  const bool lo = p.terms != 1;
+  const uint32_t planes = lo ? 2u : 1u;
+  // GN / HALO: only the B planes arrive with a stage (GN: the consumers write A themselves)
+  const uint32_t stage_tx = (GN || HALO) ? planes * Cfg::B_PLANE_BYTES : (uint32_t)(lo ? Cfg::STAGE_BYTES : Cfg::STAGE_BYTES / 2);
+  int n_idx, x0, y0, n0;
+  tc_decode(p, tile, n_idx, x0, y0, n0);
+  const int bz = p.b_batched == 1 ? n0 : 0;
+  for (int kb = kb_lo; kb < kb_hi; ++kb) {
+    int bkb = kb;   // the weights' k-block (tap-major, see tc_make_launch)
+    if constexpr (HALO) {
+      // k order (dy, slice, dx); a new A unit at dx == 0
+      const int ua = kb / halo_r, dx = kb - ua * halo_r, dy = ua / p.cb0, cs = ua - dy * p.cb0;
+      bkb = (dy * halo_r + dx) * p.cb0 + cs;
+      if (dx == 0) {
+        mbar_wait(bars.a_empty(r.aunit), r.aphase ^ 1u);
+        const uint32_t ua_s = smem_base + r.aunit * Cfg::A_UNIT_BYTES;
+        const uint32_t fa = bars.a_full(r.aunit);
+        // halo rows y0 + dy - 1 (+ the phase row), columns from x0 - 1 (+ the phase column); borders are TMA zero fill
+        const int cy = y0 + dy - 1 + p.up_py, cx = x0 - 1 + p.up_px;
+        mbar_expect_tx(fa, planes * (uint32_t)(halo_w * p.bh * 128));
+        tma_load_4d(ua_s, tm_a0h, fa, cs * BK, cx, cy, n0);
+        if (lo) tma_load_4d(ua_s + HALO_PLANE_BYTES, tm_a0l, fa, cs * BK, cx, cy, n0);
+      }
+      if (dx == halo_r - 1) {
+        if (++r.aunit == HALO_UNITS) {
+          r.aunit = 0;
+          r.aphase ^= 1u;
+        }
+      }
+    }
+    mbar_wait(bars.empty(r.stage), r.phase ^ 1u);
+    const uint32_t sa = smem_base + Cfg::A_RING_BYTES + r.stage * Cfg::STAGE_BYTES;
+    const uint32_t sb = HALO ? sa : sa + 2 * A_PLANE_BYTES;
+    const uint32_t fb = bars.full(r.stage);
+    mbar_expect_tx(fb, stage_tx);
+    if (GN || HALO) {
+    } else if (kb < p.kb0) {
+      const int tap = kb / p.cb0;
+      const int c = (kb - tap * p.cb0) * BK;
+      int cx = x0, cy = y0, cn = n0;
+      if (p.mode0 == TAPS_3X3) {
+        cy += tap / 3 - 1;
+        cx += tap % 3 - 1;
+      } else if (p.mode0 == TAPS_UP2X2) {
+        cy += tap / 2 + p.up_py - 1;
+        cx += tap % 2 + p.up_px - 1;
+      } else if (p.mode0 == TAPS_3X3_S2) {
+        const int dy = tap / 3, dx = tap % 3;
+        cy += dy >> 1;
+        cx += dx >> 1;
+        cn += ((dy & 1) * 2 + (dx & 1)) * p.phase_stride;
+      }
+      tma_load_4d(sa, tm_a0h, fb, c, cx, cy, cn);
+      if (lo) tma_load_4d(sa + A_PLANE_BYTES, tm_a0l, fb, c, cx, cy, cn);
+    } else {
+      const int c = (kb - p.kb0) * BK;
+      tma_load_4d(sa, tm_a1h, fb, c, x0, y0, n0);
+      if (lo) tma_load_4d(sa + A_PLANE_BYTES, tm_a1l, fb, c, x0, y0, n0);
+    }
+    if (PAIR) {
+      // rows [rank * BN / 2, (rank + 1) * BN / 2) of the B tile, into both CTAs (each expects the whole stage)
+      constexpr int BN = Cfg::B_PLANE_BYTES / (BK * 2);
+      const uint32_t half = rank * (BN / 2) * 128u;
+      const int brow = n_idx * BN + (int)rank * (BN / 2);
+      tma_load_3d_multicast(sb + half, tm_bh, fb, kb * BK, brow, 0, (uint16_t)3);
+      if (lo) tma_load_3d_multicast(sb + Cfg::B_PLANE_BYTES + half, tm_bl, fb, kb * BK, brow, 0, (uint16_t)3);
+    } else if (p.b_batched == 2) {
+      constexpr int BN = Cfg::B_PLANE_BYTES / (BK * 2);
+      tma_load_4d(sb, tm_bh, fb, kb * BK, n_idx * BN, y0, n0);
+      if (lo) tma_load_4d(sb + Cfg::B_PLANE_BYTES, tm_bl, fb, kb * BK, n_idx * BN, y0, n0);
+    } else {
+      constexpr int BN = Cfg::B_PLANE_BYTES / (BK * 2);
+      tma_load_3d(sb, tm_bh, fb, bkb * BK, n_idx * BN, bz);
+      if (lo) tma_load_3d(sb + Cfg::B_PLANE_BYTES, tm_bl, fb, bkb * BK, n_idx * BN, bz);
+    }
+    if (++r.stage == Cfg::STAGES) {
+      r.stage = 0;
+      r.phase ^= 1u;
+    }
+  }
+}
+
+// Epilogue of one m64 accumulator fragment: rows r0 and r0 + 8 of the output tile, 2 adjacent columns per 8-column group.
+// out = alpha * acc + chanadd + residual (res_mode 0 / 1 / 2), or alpha * acc into split-K partial `split_off`.  The stored values
+// (0 for rows past the batch) are written back to d for the GroupNorm sums.  DUAL (dual set): the hi*lo partial sums of the same
+// columns are kept BN columns further on and added first.
+template <int BN, bool DUAL, int R>
+__device__ __forceinline__ void tc_epilogue_rows(const TcParams& p, float (&d)[R], bool dual, int r0, int cq, int n_idx, int x0,
+                                                 int y0, int n0, int split_off) {
+  const int ppi = p.bw * p.bh;
+  float* orow[2];
+  const float* rrow[2];
+  const float* crow[2];
+  bool valid[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r0 + 8 * h;
+    const int xi = r % p.bw, yi = (r / p.bw) % p.bh, ni = r / ppi;
+    const int n = n0 + ni;
+    valid[h] = n < p.N;
+    orow[h] = p.out + (long long)n * p.out_sn + (long long)(y0 + yi) * p.out_sy + (long long)(x0 + xi) * p.out_sx + n_idx * BN +
+              (long long)split_off * p.split_stride;
+    rrow[h] = nullptr;
+    if (p.residual) {
+      // same pixel, nearest-upsampled (x_upd of ResBlock(up=True), unet.py:240) or the 2x2 average of a twice-as-large map
+      // (ResBlock(down=True))
+      long long rp;
+      if (p.res_mode == 0) rp = ((long long)n * p.H + (y0 + yi)) * p.W + (x0 + xi);
+      else if (p.res_mode == 1) rp = ((long long)n * (p.H >> 1) + ((y0 + yi) >> 1)) * (p.W >> 1) + ((x0 + xi) >> 1);
+      else rp = ((long long)n * (2 * p.H) + 2 * (y0 + yi)) * (2 * p.W) + 2 * (x0 + xi);
+      rrow[h] = p.residual + rp * p.ldr + n_idx * BN;
+    }
+    crow[h] = p.chanadd ? p.chanadd + (long long)n * p.ca_ld + n_idx * BN : nullptr;
+  }
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int c = 8 * j + cq;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float a0 = d[4 * j + 2 * h], a1 = d[4 * j + 2 * h + 1];
+      if constexpr (DUAL) {
+        if (dual) {   // + the hi*lo partial sums of the same columns, kept BN columns further on
+          a0 += d[4 * (j + BN / 8) + 2 * h];
+          a1 += d[4 * (j + BN / 8) + 2 * h + 1];
+        }
+      }
+      float v0 = p.alpha * a0, v1 = p.alpha * a1;
+      if (crow[h] && valid[h]) {
+        const float2 cv = __ldg(reinterpret_cast<const float2*>(crow[h] + c));
+        v0 += cv.x;
+        v1 += cv.y;
+      }
+      if (rrow[h] && valid[h]) {
+        float2 rv = __ldg(reinterpret_cast<const float2*>(rrow[h] + c));
+        if (p.res_mode == 2) {
+          const long long r_dx = p.ldr, r_dy = (long long)2 * p.W * p.ldr;
+          const float2 q1 = __ldg(reinterpret_cast<const float2*>(rrow[h] + r_dx + c));
+          const float2 q2 = __ldg(reinterpret_cast<const float2*>(rrow[h] + r_dy + c));
+          const float2 q3 = __ldg(reinterpret_cast<const float2*>(rrow[h] + r_dy + r_dx + c));
+          rv.x = ((rv.x + q1.x) + (q2.x + q3.x)) * 0.25f;
+          rv.y = ((rv.y + q1.y) + (q2.y + q3.y)) * 0.25f;
+        }
+        v0 += rv.x;
+        v1 += rv.y;
+      }
+      if (!valid[h]) v0 = v1 = 0.f;
+      d[4 * j + 2 * h] = v0;
+      d[4 * j + 2 * h + 1] = v1;
+      if (valid[h]) *reinterpret_cast<float2*>(orow[h] + c) = make_float2(v0, v1);
+    }
+  }
+}
+
+// GroupNorm sums, step 1: the column sums and sums of squares of one warp's 16 rows of a fragment (after tc_epilogue_rows), reduced
+// across the 8 lanes that share a column pair, into part[BN] of that 16-row group
+template <int BN, int R>
+__device__ __forceinline__ void tc_stats_rows(const float (&d)[R], float2* part, int lane, int cq) {
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const float a = d[4 * j + e], b = d[4 * j + 2 + e];
+      float s = a + b, q = a * a + b * b;
+#pragma unroll
+      for (int k = 4; k <= 16; k <<= 1) {
+        s += __shfl_xor_sync(0xffffffffu, s, k);
+        q += __shfl_xor_sync(0xffffffffu, q, k);
+      }
+      if (lane < 4) part[8 * j + cq + e] = make_float2(s, q);
+    }
+  }
+}
+
 template <int BN, bool PAIR, bool DUAL, bool GN, bool HALO>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant__ CUtensorMap tm_a0l,
@@ -116,10 +332,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_base = smem_base + Cfg::RING_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto a_full_bar = [&](int u) { return bar_base + 8u * (2 * STAGES + u); };                // HALO: A units
-  auto a_empty_bar = [&](int u) { return bar_base + 8u * (2 * STAGES + HALO_UNITS + u); };
+  const TcBars<STAGES> bars{bar_base};
+  auto full_bar = [&](int s) { return bars.full(s); };
+  auto empty_bar = [&](int s) { return bars.empty(s); };
+  auto a_full_bar = [&](int u) { return bars.a_full(u); };     // HALO: A units
+  auto a_empty_bar = [&](int u) { return bars.a_empty(u); };
   // HALO: k-blocks per A unit of the source-0 taps (the dx taps of one dy) and the unit's pixels per row
   const int halo_r = p.mode0 == TAPS_UP2X2 ? 2 : 3;
   const int halo_w = p.bw + halo_r - 1;
@@ -186,103 +403,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
   if (PAIR) cluster_sync_all();   // the peer's barriers exist before any multicast or remote arrive can reach them
   else __syncthreads();
 
-  auto decode = [&](int tile, int& n_idx, int& x0, int& y0, int& n0) {
-    n_idx = tile % p.n_tiles;
-    int m = tile / p.n_tiles;
-    int tx = m % p.tiles_x;
-    int t2 = m / p.tiles_x;
-    int ty = t2 % p.tiles_y;
-    int tn = t2 / p.tiles_y;
-    x0 = tx * p.bw;
-    y0 = ty * p.bh;
-    n0 = tn * p.bn;
-  };
+  auto decode = [&](int tile, int& n_idx, int& x0, int& y0, int& n0) { tc_decode(p, tile, n_idx, x0, y0, n0); };
 
   if (warp == 8) {
     // ------------------------------------------------ TMA producer ------------------------------------------------
     if (lane == 0) {
-      uint32_t stage = 0, phase = 0;
-      uint32_t aunit = 0, aphase = 0;   // HALO: A ring position
-      const bool lo = p.terms != 1;
-      const uint32_t planes = lo ? 2u : 1u;
-      // GN / HALO: only the B planes arrive with a stage (GN: the consumers write A themselves)
-      const uint32_t stage_tx = (GN || HALO) ? planes * Cfg::B_PLANE_BYTES : (uint32_t)(lo ? Cfg::STAGE_BYTES : Cfg::STAGE_BYTES / 2);
-      for (int u = unit_begin; u < unit_end; u += unit_step) {
-        int n_idx, x0, y0, n0;
-        decode(tile_of(u), n_idx, x0, y0, n0);
-        const int bz = p.b_batched == 1 ? n0 : 0;
-        const int kb_lo = k_lo(u), kb_hi = k_hi(u);
-        for (int kb = kb_lo; kb < kb_hi; ++kb) {
-          int bkb = kb;   // the weights' k-block (tap-major, see tc_make_launch)
-          if constexpr (HALO) {
-            // k order (dy, slice, dx); a new A unit at dx == 0
-            const int ua = kb / halo_r, dx = kb - ua * halo_r, dy = ua / p.cb0, cs = ua - dy * p.cb0;
-            bkb = (dy * halo_r + dx) * p.cb0 + cs;
-            if (dx == 0) {
-              mbar_wait(a_empty_bar(aunit), aphase ^ 1u);
-              const uint32_t ua_s = smem_base + aunit * Cfg::A_UNIT_BYTES;
-              const uint32_t fa = a_full_bar(aunit);
-              // halo rows y0 + dy - 1 (+ the phase row), columns from x0 - 1 (+ the phase column); borders are TMA zero fill
-              const int cy = y0 + dy - 1 + p.up_py, cx = x0 - 1 + p.up_px;
-              mbar_expect_tx(fa, planes * (uint32_t)(halo_w * p.bh * 128));
-              tma_load_4d(ua_s, &tm_a0h, fa, cs * BK, cx, cy, n0);
-              if (lo) tma_load_4d(ua_s + HALO_PLANE_BYTES, &tm_a0l, fa, cs * BK, cx, cy, n0);
-            }
-            if (dx == halo_r - 1) {
-              if (++aunit == HALO_UNITS) {
-                aunit = 0;
-                aphase ^= 1u;
-              }
-            }
-          }
-          mbar_wait(empty_bar(stage), phase ^ 1u);
-          const uint32_t sa = smem_base + Cfg::A_RING_BYTES + stage * Cfg::STAGE_BYTES;
-          const uint32_t sb = HALO ? sa : sa + 2 * A_PLANE_BYTES;
-          const uint32_t fb = full_bar(stage);
-          mbar_expect_tx(fb, stage_tx);
-          if (GN || HALO) {
-          } else if (kb < p.kb0) {
-            const int tap = kb / p.cb0;
-            const int c = (kb - tap * p.cb0) * BK;
-            int cx = x0, cy = y0, cn = n0;
-            if (p.mode0 == TAPS_3X3) {
-              cy += tap / 3 - 1;
-              cx += tap % 3 - 1;
-            } else if (p.mode0 == TAPS_UP2X2) {
-              cy += tap / 2 + p.up_py - 1;
-              cx += tap % 2 + p.up_px - 1;
-            } else if (p.mode0 == TAPS_3X3_S2) {
-              const int dy = tap / 3, dx = tap % 3;
-              cy += dy >> 1;
-              cx += dx >> 1;
-              cn += ((dy & 1) * 2 + (dx & 1)) * p.phase_stride;
-            }
-            tma_load_4d(sa, &tm_a0h, fb, c, cx, cy, cn);
-            if (lo) tma_load_4d(sa + A_PLANE_BYTES, &tm_a0l, fb, c, cx, cy, cn);
-          } else {
-            const int c = (kb - p.kb0) * BK;
-            tma_load_4d(sa, &tm_a1h, fb, c, x0, y0, n0);
-            if (lo) tma_load_4d(sa + A_PLANE_BYTES, &tm_a1l, fb, c, x0, y0, n0);
-          }
-          if (PAIR) {
-            // rows [rank * BN / 2, (rank + 1) * BN / 2) of the B tile, into both CTAs (each expects the whole stage)
-            const uint32_t half = (uint32_t)rank * (BN / 2) * 128u;
-            const int brow = n_idx * BN + (int)rank * (BN / 2);
-            tma_load_3d_multicast(sb + half, &tm_bh, fb, kb * BK, brow, 0, (uint16_t)3);
-            if (lo) tma_load_3d_multicast(sb + Cfg::B_PLANE_BYTES + half, &tm_bl, fb, kb * BK, brow, 0, (uint16_t)3);
-          } else if (p.b_batched == 2) {
-            tma_load_4d(sb, &tm_bh, fb, kb * BK, n_idx * BN, y0, n0);
-            if (lo) tma_load_4d(sb + Cfg::B_PLANE_BYTES, &tm_bl, fb, kb * BK, n_idx * BN, y0, n0);
-          } else {
-            tma_load_3d(sb, &tm_bh, fb, bkb * BK, n_idx * BN, bz);
-            if (lo) tma_load_3d(sb + Cfg::B_PLANE_BYTES, &tm_bl, fb, bkb * BK, n_idx * BN, bz);
-          }
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-      }
+      TcRing ring;
+      for (int u = unit_begin; u < unit_end; u += unit_step)
+        tc_produce_tile<Cfg, PAIR, GN, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars, tile_of(u), k_lo(u),
+                                             k_hi(u), rank, ring);
     }
   } else {
   // ------------------------------------------------ consumers: wgmma + epilogue ------------------------------------------------
@@ -457,88 +586,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
     // ---- epilogue: rows r0 and r0 + 8 of this tile, 2 adjacent columns per 8-column group ----
     int n_idx, x0, y0, n0;
     decode(tile_of(u), n_idx, x0, y0, n0);
-    const int split_off = PAIR ? 0 : u % p.split_k;
-    float* orow[2];
-    const float* rrow[2];
-    const float* crow[2];
-    bool valid[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int r = r0 + 8 * h;
-      const int xi = r % p.bw, yi = (r / p.bw) % p.bh, ni = r / ppi;
-      const int n = n0 + ni;
-      valid[h] = n < p.N;
-      orow[h] = p.out + (long long)n * p.out_sn + (long long)(y0 + yi) * p.out_sy + (long long)(x0 + xi) * p.out_sx + n_idx * BN +
-                (long long)split_off * p.split_stride;
-      rrow[h] = nullptr;
-      if (p.residual) {
-        // same pixel, nearest-upsampled (x_upd of ResBlock(up=True), unet.py:240) or the 2x2 average of a twice-as-large map
-        // (ResBlock(down=True))
-        long long rp;
-        if (p.res_mode == 0) rp = ((long long)n * p.H + (y0 + yi)) * p.W + (x0 + xi);
-        else if (p.res_mode == 1) rp = ((long long)n * (p.H >> 1) + ((y0 + yi) >> 1)) * (p.W >> 1) + ((x0 + xi) >> 1);
-        else rp = ((long long)n * (2 * p.H) + 2 * (y0 + yi)) * (2 * p.W) + 2 * (x0 + xi);
-        rrow[h] = p.residual + rp * p.ldr + n_idx * BN;
-      }
-      crow[h] = p.chanadd ? p.chanadd + (long long)n * p.ca_ld + n_idx * BN : nullptr;
-    }
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int c = 8 * j + cq;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float a0 = d[4 * j + 2 * h], a1 = d[4 * j + 2 * h + 1];
-        if constexpr (DUAL) {
-          if (dual) {   // + the hi*lo partial sums of the same columns, kept BN columns further on
-            a0 += d[4 * (j + BN / 8) + 2 * h];
-            a1 += d[4 * (j + BN / 8) + 2 * h + 1];
-          }
-        }
-        float v0 = p.alpha * a0, v1 = p.alpha * a1;
-        if (crow[h] && valid[h]) {
-          const float2 cv = __ldg(reinterpret_cast<const float2*>(crow[h] + c));
-          v0 += cv.x;
-          v1 += cv.y;
-        }
-        if (rrow[h] && valid[h]) {
-          float2 rv = __ldg(reinterpret_cast<const float2*>(rrow[h] + c));
-          if (p.res_mode == 2) {
-            const long long r_dx = p.ldr, r_dy = (long long)2 * p.W * p.ldr;
-            const float2 q1 = __ldg(reinterpret_cast<const float2*>(rrow[h] + r_dx + c));
-            const float2 q2 = __ldg(reinterpret_cast<const float2*>(rrow[h] + r_dy + c));
-            const float2 q3 = __ldg(reinterpret_cast<const float2*>(rrow[h] + r_dy + r_dx + c));
-            rv.x = ((rv.x + q1.x) + (q2.x + q3.x)) * 0.25f;
-            rv.y = ((rv.y + q1.y) + (q2.y + q3.y)) * 0.25f;
-          }
-          v0 += rv.x;
-          v1 += rv.y;
-        }
-        if (!valid[h]) v0 = v1 = 0.f;
-        d[4 * j + 2 * h] = v0;
-        d[4 * j + 2 * h + 1] = v1;
-        if (valid[h]) *reinterpret_cast<float2*>(orow[h] + c) = make_float2(v0, v1);
-      }
-    }
+    tc_epilogue_rows<BN, DUAL>(p, d, dual, r0, cq, n_idx, x0, y0, n0, PAIR ? 0 : u % p.split_k);
     if (p.stats) {
       // GroupNorm statistics of the tile.  (1) per warp: the column sums over its 16 rows (one image: >= 32 pixels per image),
       // reduced across the 8 lanes that share a column pair; (2) per image slot: the warps of that image added in a fixed order
       // into running (value, compensation) pairs that persist while consecutive tiles of this CTA stay in the same image and
       // channel block (the tile -> CTA map is static, so these fp32 partial sums are the same every run); (3) flushed with one
       // order-independent fixed-point add per value otherwise
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float a = d[4 * j + e], b = d[4 * j + 2 + e];
-          float s = a + b, q = a * a + b * b;
-#pragma unroll
-          for (int k = 4; k <= 16; k <<= 1) {
-            s += __shfl_xor_sync(0xffffffffu, s, k);
-            q += __shfl_xor_sync(0xffffffffu, q, k);
-          }
-          if (lane < 4) part[warp * BN + 8 * j + cq + e] = make_float2(s, q);
-        }
-      }
+      tc_stats_rows<BN>(d, part + warp * BN, lane, cq);
       named_bar_sync(1, kConsumerThreads);
       const int nslots = 8 / wpi;
       bool flush = true;
@@ -572,6 +627,235 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
   }
   __syncwarp();                   // the producer warp's lane 0 leaves its loop before the aligned cluster barrier
   if (PAIR) cluster_sync_all();   // no multicast or remote arrive may reach a CTA that has exited
+}
+
+// -------------------------------------------------------------------------------------------------------------------
+// Ping-pong form: 3 warpgroups.  WG0 is the TMA producer (one elected thread, 40 registers per thread); WG1 and WG2 are consumers
+// (232 registers) that each own a WHOLE 128-row tile as two m64 x BN fragments and take turns on the tensor cores: the units of a
+// CTA alternate between them, and an ordered turn (one mbarrier per consumer) lets only one warpgroup issue wgmma at a time, in
+// tile order.  A warpgroup hands the turn over right after issuing its last k-block, then waits for its MMAs, releases the stages
+// and runs the epilogue while the other warpgroup's MMAs keep the tensor cores busy.  Each output element gets the products of the
+// three-instruction form in the same order (hi*hi, hi*lo, lo*hi per 16-deep k-step), so the output is bit-identical to
+// conv_tc_kernel without DUAL.  Used for the single-CTA launches without the GN form where a CTA walks at least two tiles.
+// -------------------------------------------------------------------------------------------------------------------
+static constexpr int kPpThreads = 384;
+
+template <int BN, bool HALO>
+struct PpCfg {
+  using Ring = TcCfg<BN, false, HALO>;   // the ring layout of conv_tc_kernel (no DUAL: it only changes the accumulator)
+  // GroupNorm sums, per consumer warpgroup: per-16-row-group column partials (8 groups x BN x {sum, sumsq}) and one running
+  // (value, compensation) pair per {sum, sumsq} x BN column — carried across tiles only when the tile is one image (see the
+  // epilogue), so one image slot suffices
+  static constexpr int PART_BYTES = 8 * BN * 8;
+  static constexpr int RUN_BYTES = 2 * BN * 8;
+  static constexpr int STAT_BYTES = PART_BYTES + RUN_BYTES;
+  static constexpr int SMEM_BYTES = Ring::RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * STAT_BYTES;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory capacity");
+};
+
+template <int BN, int TERMS, bool HALO>
+__global__ void __launch_bounds__(kPpThreads, 1)
+conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant__ CUtensorMap tm_a0l,
+                        const __grid_constant__ CUtensorMap tm_a1h, const __grid_constant__ CUtensorMap tm_a1l,
+                        const __grid_constant__ CUtensorMap tm_bh, const __grid_constant__ CUtensorMap tm_bl, const TcParams p) {
+  static_assert(TERMS == 1 || TERMS == 3, "1 or 3 fp16 products per MAC");
+  using Cfg = PpCfg<BN, HALO>;
+  using Ring = typename Cfg::Ring;
+  constexpr int STAGES = Ring::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const TcBars<STAGES> bars{smem_base + Ring::RING_BYTES};
+
+  pdl_prologue();
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int KB = p.kb0 + p.kb1;
+  const int n_units = p.tiles_x * p.tiles_y * p.tiles_n * p.n_tiles * p.split_k;
+  const int n_workers = (int)gridDim.x, worker = (int)blockIdx.x;
+  // the tile -> CTA deal of conv_tc_kernel
+  const int unit_begin = p.deal ? (int)((long long)worker * n_units / n_workers) : worker;
+  const int unit_end = p.deal ? (int)((long long)(worker + 1) * n_units / n_workers) : n_units;
+  const int unit_step = p.deal ? 1 : n_workers;
+  auto k_lo = [&](int u) { return (int)((long long)(u % p.split_k) * KB / p.split_k); };
+  auto k_hi = [&](int u) { return (int)((long long)(u % p.split_k + 1) * KB / p.split_k); };
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tm_a0h);
+    tma_prefetch_desc(&tm_a0l);
+    tma_prefetch_desc(&tm_bh);
+    tma_prefetch_desc(&tm_bl);
+    if (p.kb1) {
+      tma_prefetch_desc(&tm_a1h);
+      tma_prefetch_desc(&tm_a1l);
+    }
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(bars.full(s), 1);    // the producer's expect_tx arrive
+      mbar_init(bars.empty(s), 4);   // one arrive per warp of the consuming warpgroup
+    }
+    if (HALO) {
+      for (int u = 0; u < HALO_UNITS; ++u) {
+        mbar_init(bars.a_full(u), 1);
+        mbar_init(bars.a_empty(u), 4);
+      }
+    }
+    mbar_init(bars.turn(0), 4);   // consumer c may issue its next tile's MMAs: the 4 warps of the other one have issued theirs
+    mbar_init(bars.turn(1), 4);
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ------------------------------------------------ TMA producer ------------------------------------------------
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      TcRing ring;
+      for (int u = unit_begin; u < unit_end; u += unit_step)
+        tc_produce_tile<Ring, false, false, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars,
+                                                  u / p.split_k, k_lo(u), k_hi(u), 0u, ring);
+    }
+    return;
+  }
+  // ------------------------------------------------ consumers: wgmma + epilogue ------------------------------------------------
+  setmaxnreg_inc<232>();
+  const int c = (warp >> 2) - 1;          // consumer warpgroup: units c, c + 2, ... of this CTA
+  const int wq = warp & 3;
+  const int tid = threadIdx.x - 128 * (c + 1);
+  // fragment f holds tile rows [64 f, 64 f + 64); a thread holds, for every 8-column group j, columns 8j + 2(lane % 4) + {0, 1} of
+  // rows 64 f + r0 (d[f][4j], d[f][4j+1]) and 64 f + r0 + 8 (d[f][4j+2], d[f][4j+3])
+  const int r0 = wq * 16 + (lane >> 2);
+  const int cq = (lane & 3) * 2;
+  const int halo_r = p.mode0 == TAPS_UP2X2 ? 2 : 3;
+  const int halo_w = p.bw + halo_r - 1;
+  const int units_per_tile = p.cb0 * halo_r;   // HALO: A units per tile
+  // HALO: the first pixel (yi, xi) of fragment f inside the tile, as a row of the halo unit
+  uint32_t halo_row_off[2];
+#pragma unroll
+  for (int f = 0; f < 2; ++f) halo_row_off[f] = (uint32_t)(((f * 64) / p.bw) * halo_w + (f * 64) % p.bw) * 128u;
+  const int wpi = p.bw * p.bh >= 128 ? 8 : p.bw * p.bh / 16;   // 16-row groups per image slot of the tile
+  uint8_t* stat_smem = smem_raw + (bars.base + 256u - smem_u32(smem_raw)) + c * Cfg::STAT_BYTES;
+  float2* part = reinterpret_cast<float2*>(stat_smem);                     // [16-row group][BN] {sum, sumsq}
+  float2* run = reinterpret_cast<float2*>(stat_smem + Cfg::PART_BYTES);    // [which][BN] {value, compensation}
+  if (p.stats) {
+    for (int i = tid; i < 2 * BN; i += 128) run[i] = make_float2(0.f, 0.f);
+  }
+  auto release = [&](int s) {
+    if (lane == 0) mbar_arrive(bars.empty(s));
+  };
+  auto release_a = [&](uint32_t a) {
+    if (lane == 0) mbar_arrive(bars.a_empty(a % HALO_UNITS));
+  };
+  // position of this warpgroup's next k-block in the B-stage ring: all k-blocks of the CTA's earlier units, both warpgroups'
+  uint32_t kpos = c ? (uint32_t)(k_hi(unit_begin) - k_lo(unit_begin)) : 0u;
+  float d[2][BN / 2];
+  int turn = 0;
+  for (int u = unit_begin + c * unit_step; u < unit_end; u += 2 * unit_step, ++turn) {
+    const int kb_lo = k_lo(u), kb_hi = k_hi(u);
+    if (c == 1 || turn > 0) mbar_wait(bars.turn(c), (uint32_t)(c ? turn : turn - 1) & 1u);
+    uint32_t stage = kpos % STAGES, phase = (kpos / STAGES) & 1u;
+    const uint32_t a_done = (uint32_t)((2 * turn + c) * units_per_tile);   // HALO: A units of the CTA's earlier tiles
+    int prev = -1;
+    for (int kb = kb_lo; kb < kb_hi; ++kb) {
+      const uint32_t sb = smem_base + Ring::A_RING_BYTES + stage * Ring::STAGE_BYTES;
+      uint32_t a_base = sb;   // fragment 0's rows of the A_hi plane
+      uint32_t a_frag1 = 64u * 128u;
+      uint32_t a_plane = A_PLANE_BYTES;
+      uint32_t a_unit = 0;
+      bool a_first = false;
+      if constexpr (HALO) {
+        // HALO launches have no side input: k-block kb reads unit kb / halo_r, shifted by dx pixels
+        const int ua = halo_r == 3 ? (int)(__umulhi((uint32_t)kb, 0xAAAAAAABu) >> 1) : kb >> 1;
+        const int dx = kb - ua * halo_r;
+        a_unit = a_done + (uint32_t)ua;
+        a_first = dx == 0;
+        if (a_first) mbar_wait(bars.a_full(a_unit % HALO_UNITS), (a_unit / HALO_UNITS) & 1u);
+        a_base = smem_base + (a_unit % HALO_UNITS) * Ring::A_UNIT_BYTES + halo_row_off[0] + 128u * dx;
+        a_frag1 = halo_row_off[1] - halo_row_off[0];
+        a_plane = HALO_PLANE_BYTES;
+      }
+      mbar_wait(bars.full(stage), phase);
+      const uint32_t sbb = HALO ? sb : sb + 2 * A_PLANE_BYTES;
+      const uint64_t ah0 = wgmma_desc_sw128(a_base), ah1 = wgmma_desc_sw128(a_base + a_frag1);
+      const uint64_t al0 = wgmma_desc_sw128(a_base + a_plane), al1 = wgmma_desc_sw128(a_base + a_frag1 + a_plane);
+      const uint64_t bh = wgmma_desc_sw128(sbb);
+      const uint64_t bl = wgmma_desc_sw128(sbb + Ring::B_PLANE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t adv = 2u * k;   // 16 fp16 = 32 bytes = 2 x 16-byte units inside the swizzle row
+        const uint32_t acc = (uint32_t)(kb != kb_lo || k != 0);
+        wgmma_tile<BN>(d[0], ah0 + adv, bh + adv, acc);
+        wgmma_tile<BN>(d[1], ah1 + adv, bh + adv, acc);
+        if constexpr (TERMS == 3) {
+          wgmma_tile<BN>(d[0], ah0 + adv, bl + adv, 1u);
+          wgmma_tile<BN>(d[1], ah1 + adv, bl + adv, 1u);
+          wgmma_tile<BN>(d[0], al0 + adv, bh + adv, 1u);
+          wgmma_tile<BN>(d[1], al1 + adv, bh + adv, 1u);
+        }
+      }
+      wgmma_commit();
+      // the previous k-block's group has completed once at most this one is pending: its stage goes back to the producer
+      wgmma_wait<1>();
+      if (prev >= 0) release(prev);
+      prev = (int)stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1u;
+      }
+      // and so has the previous A unit if that k-block was its last reader (this one opens a new unit)
+      if (HALO && a_first && kb != kb_lo) release_a(a_unit - 1);
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bars.turn(c ^ 1));   // every MMA of this tile is issued: the other warpgroup's turn
+    wgmma_wait<0>();
+    if (prev >= 0) release(prev);
+    if (HALO) release_a(a_done + units_per_tile - 1);
+    // the other warpgroup's unit (if any) lies between this one and this warpgroup's next in the ring
+    kpos += (uint32_t)(kb_hi - kb_lo) + (uint32_t)(k_hi(u + unit_step) - k_lo(u + unit_step));
+
+    // ---- epilogue ----
+    int n_idx, x0, y0, n0;
+    tc_decode(p, u / p.split_k, n_idx, x0, y0, n0);
+#pragma unroll
+    for (int f = 0; f < 2; ++f) tc_epilogue_rows<BN, false>(p, d[f], false, 64 * f + r0, cq, n_idx, x0, y0, n0, u % p.split_k);
+    if (p.stats) {
+      // GroupNorm statistics of the tile, as in conv_tc_kernel: (1) per 16-row group (warp wq of fragment f = group 4 f + wq), the
+      // column sums, (2) per image slot the groups of that image in a fixed order, into a running (value, compensation) pair that
+      // persists while this warpgroup's consecutive tiles stay in one image and channel block (only possible when a tile is one
+      // image), (3) flushed with one fixed-point add per value otherwise
+#pragma unroll
+      for (int f = 0; f < 2; ++f) tc_stats_rows<BN>(d[f], part + (4 * f + wq) * BN, lane, cq);
+      named_bar_sync(1 + c, 128);
+      const int nslots = 8 / wpi;
+      bool flush = true;
+      const int un = u + 2 * unit_step;   // this warpgroup's next unit
+      if (un < unit_end) {
+        int nn_idx, nx0, ny0, nn0;
+        tc_decode(p, un / p.split_k, nn_idx, nx0, ny0, nn0);
+        flush = nslots > 1 || nn0 != n0 || nn_idx != n_idx;
+      }
+      for (int i = tid; i < 2 * BN; i += 128) {
+        const int which = i / BN, col = i - which * BN;
+        for (int g = 0; g < nslots; ++g) {
+          float2 acc = nslots == 1 ? run[i] : make_float2(0.f, 0.f);
+          for (int w = g * wpi; w < (g + 1) * wpi; ++w) {
+            const float2 pv = part[w * BN + col];
+            two_sum_acc(acc.x, acc.y, which ? pv.y : pv.x);
+          }
+          if (flush) {
+            const int n = n0 + g;
+            if (n < p.N) {
+              StatAcc* dst = p.stats + ((size_t)n * p.st_ld + n_idx * BN + col) * 2 + which;
+              stat_add(dst, acc.x);   // integer accumulation: the total is independent of the arrival order
+              stat_add(dst, acc.y);
+            }
+            acc = make_float2(0.f, 0.f);
+          }
+          if (nslots == 1) run[i] = acc;
+        }
+      }
+      named_bar_sync(1 + c, 128);   // part[] is rewritten by this warpgroup's next tile
+    }
+  }
 }
 
 // -------------------------------------------------------------------------------------------------------------------
@@ -637,6 +921,10 @@ void tc_debug_pair_dual(int on) { g_pair_dual = on; }
 // HALO form wherever legal (see tc_make_launch); env DDNM_HALO=0 / tc_debug_halo(0) keep every launch on one A load per k-block
 static int g_halo_enable = [] { const char* v = std::getenv("DDNM_HALO"); return v && *v ? std::atoi(v) : 1; }();
 void tc_debug_halo(int on) { g_halo_enable = on; }
+// ping-pong kernel for the single-CTA launches without the GN form (see tc_run); env DDNM_PINGPONG=0 / tc_debug_pingpong(0) keep
+// them on conv_tc_kernel
+static int g_pingpong_enable = [] { const char* v = std::getenv("DDNM_PINGPONG"); return v && *v ? std::atoi(v) : 1; }();
+void tc_debug_pingpong(int on) { g_pingpong_enable = on; }
 static int g_deal = -1;
 void tc_debug_deal(int mode) {
   DDNM_CHECK(mode >= -1 && mode <= 1, "deal mode must be -1 (default rule), 0 (round-robin) or 1 (contiguous ranges)");
@@ -678,6 +966,7 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
     L.pair = g_pair_mode == 1 && w_batches == 1 && m_tiles % 2 == 0;
   }
   L.dual = g_dual_mode != 0 && (!L.pair || g_pair_dual != 0);
+  L.pingpong = g_pingpong_enable != 0;
   p.mode0 = mode0;
   p.cb0 = src0.C / BK;
   p.kb0 = taps * p.cb0;
@@ -771,6 +1060,7 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
   L.BN = 64;
   if (N % 128 == 0 && (long long)m_tiles * (N / 128) >= num_sms / 2) L.BN = 128;
   L.dual = g_dual_mode != 0;
+  L.pingpong = g_pingpong_enable != 0;
   p.n_tiles = N / L.BN;
   p.mode0 = TAPS_1X1;
   p.cb0 = K / BK; p.kb0 = K / BK; p.kb1 = 0;
@@ -821,6 +1111,28 @@ static void launch_forms(const TcLaunch& L, cudaStream_t stream) {
   else if (L.pair) launch_bn<BN, true, false>(L, stream);
   else if (L.dual) launch_bn<BN, false, true>(L, stream);
   else launch_bn<BN, false, false>(L, stream);
+}
+
+template <int BN, int TERMS, bool HALO>
+static void launch_pingpong(const TcLaunch& L, cudaStream_t stream) {
+  using Cfg = PpCfg<BN, HALO>;
+  static bool attr_set[64] = {};
+  if (first_use_on_device(attr_set))
+    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_pingpong_kernel<BN, TERMS, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+  launch_pdl(conv_tc_pingpong_kernel<BN, TERMS, HALO>, dim3(L.grid), dim3(kPpThreads), (size_t)Cfg::SMEM_BYTES, stream, 1,
+             HALO ? L.hh : L.a0h, HALO ? L.hl : L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.p);
+  CUDA_CHECK(cudaGetLastError());
+}
+
+template <int BN>
+static void launch_pingpong_forms(const TcLaunch& L, cudaStream_t stream) {
+  if (L.p.terms == 1) {
+    if (L.halo) launch_pingpong<BN, 1, true>(L, stream);
+    else launch_pingpong<BN, 1, false>(L, stream);
+  } else {
+    if (L.halo) launch_pingpong<BN, 3, true>(L, stream);
+    else launch_pingpong<BN, 3, false>(L, stream);
+  }
 }
 
 // ---- GN form: fused GroupNorm + SiLU + split + 3x3 convolution ----
@@ -876,6 +1188,16 @@ void tc_run(const TcLaunch& L, cudaStream_t stream) {
   DDNM_CHECK(!L.pair || L.p.split_k == 1, "CTA pairs do not split K");
   DDNM_CHECK(!L.halo || (L.p.split_k == 1 && !L.pair && !L.gn && L.p.kb1 == 0),
              "the HALO form runs unsplit single-CTA launches with TMA-loaded A and no 1x1 side input");
+  // ping-pong needs two tiles per CTA to overlap one tile's epilogue with the next one's MMAs; a CTA with one tile (the split-K
+  // launches, the 16x16 level) runs faster on two warpgroups sharing it
+  const int units = L.p.tiles_x * L.p.tiles_y * L.p.tiles_n * L.p.n_tiles * L.p.split_k;
+  if (L.pingpong && !L.pair && !L.gn && units > L.grid) {
+    switch (L.BN) {
+      case 128: launch_pingpong_forms<128>(L, stream); return;
+      case 64: launch_pingpong_forms<64>(L, stream); return;
+      default: throw Error("bad BN");
+    }
+  }
   switch (L.BN) {
     case 128: launch_forms<128>(L, stream); break;
     case 64: launch_forms<64>(L, stream); break;

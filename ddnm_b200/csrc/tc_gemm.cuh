@@ -67,6 +67,7 @@ struct TcLaunch {
   bool dual = false;           // A_hi x [B_hi; B_lo] as one m64 x 2BN instruction, two partial accumulators
   bool gn = false;             // GN form: A produced in the kernel from g
   bool halo = false;           // HALO form: one A load per (dy, channel slice) feeds the dx taps; needs split_k == 1
+  bool pingpong = false;       // ping-pong kernel where the launch allows it (see tc_run); DUAL does not apply there
   TcGnArgs g;
   int grid = 0;
   double flops = 0;            // algorithmic flops (2*M*N*K, counted once)
@@ -119,6 +120,7 @@ void tc_debug_pair_mode(int mode);   // -1 (default) / 0: no CTA pairs, 1: CTA p
 void tc_debug_dual_mode(int mode);   // 1 (default): DUAL form for single-CTA launches, 0: never
 void tc_debug_pair_dual(int on);     // 1 (default): CTA pairs use the DUAL form too, 0: the plain pair form
 void tc_debug_halo(int on);          // 1 (default, env DDNM_HALO): HALO form wherever legal, 0: never
+void tc_debug_pingpong(int on);      // 1 (default, env DDNM_PINGPONG): ping-pong kernel wherever it applies, 0: never
 // number of fp16 product terms used by launches built from now on (3 = parity mode, 1 = fast mode)
 void tc_set_terms(int terms);
 int tc_get_terms();

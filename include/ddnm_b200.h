@@ -254,6 +254,10 @@ int ddnm_tc_debug_pair_dual(int on);
  * a 1x1 side input load each
  * (dy, 64-channel slice) of the activation once as halo rows for all column taps; 0: one A load per tap */
 int ddnm_tc_debug_halo(int on);
+/* 1 (default, also env DDNM_PINGPONG): single-CTA launches without the fused GroupNorm form, built afterwards, run on the ping-pong
+ * kernel (two consumer warpgroups that each own a whole tile and take turns on the tensor cores) where a CTA gets at least two tiles;
+ * 0: never */
+int ddnm_tc_debug_pingpong(int on);
 
 #ifdef __cplusplus
 }

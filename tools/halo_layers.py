@@ -1,13 +1,15 @@
-"""Where the HALO form of the wgmma convolution moves time, layer by layer, on the celeba `Model` at B = 16 (the bench workload).
+"""Where a form of the wgmma convolution moves time, layer by layer, on the celeba `Model` at B = 16 (the bench workload).
+--switch halo (default): the HALO form; --switch pingpong: the ping-pong kernel.
 
 1. Every celeba layer shape the HALO form applies to (3x3 stride 1 and upsample phases on maps >= 64 px wide), timed with
    `ddnm_conv_tc_bench` on pseudo-random operands, the form off and on alternately: ms, algorithmic TFLOP/s and the L2 -> shared
-   memory fill bytes per launch computed from the shape.
+   memory fill bytes per launch computed from the shape (HALO).  With --switch pingpong the epilogue features are the network's
+   (GroupNorm sums, residual, channel add).
 2. One eager forward per arm (`Model.profile`, CUDA events around every launch), twice per arm in alternation: per tensor-core launch
    ms both ways, and the totals.
 
 The GPU's name, power limit and SM clocks are printed with the numbers (read-only nvidia-smi queries).
-Usage: python tools/halo_layers.py [--iters 20] [--json OUT]"""
+Usage: python tools/halo_layers.py [--switch halo|pingpong] [--iters 20] [--json OUT]"""
 import argparse
 import ctypes as C
 import json
@@ -41,7 +43,8 @@ SHAPES = [
     ("up2 128->256 128ch (phase)", 128, 128, 128, True),
     ("up2 64->128 256ch (phase)", 64, 256, 256, True),
 ]
-FEAT_STATS, FEAT_UP2 = 16, 128   # ddnm_conv_tc_bench mode bits: GroupNorm sums of the output, upsample phase
+FEAT_STATS, FEAT_RES, FEAT_CHANADD, FEAT_UP2 = 16, 32, 64, 128   # ddnm_conv_tc_bench mode bits (see api.cu)
+SWITCHES = {"halo": "ddnm_tc_debug_halo", "pingpong": "ddnm_tc_debug_pingpong"}
 
 
 def gpu_info():
@@ -64,18 +67,21 @@ def fill_bytes(H, W, Cin, Cout, up2, halo, bn=128):
     return tiles * (a + b)
 
 
-def bench_shapes(L, iters):
+def bench_shapes(L, switch, iters):
     ms, fl = C.c_float(), C.c_double()
     rows = []
     for label, H, Cin, Cout, up2 in SHAPES:
-        mode = FEAT_STATS | (FEAT_UP2 if up2 else 0)   # 3x3 stride 1 (mode 0) + the epilogue features the network uses
+        # 3x3 stride 1 (mode 0) + the epilogue features the network uses (the op-level upsample phase takes no residual)
+        mode = FEAT_STATS | (FEAT_UP2 if up2 else 0)
+        if switch == "ddnm_tc_debug_pingpong":
+            mode |= FEAT_CHANADD | (0 if up2 else FEAT_RES)
         t = {0: [], 1: []}
         for rep in range(2):
             for halo in (0, 1):
-                _lib.check(L.ddnm_tc_debug_halo(halo))
+                _lib.check(getattr(L, switch)(halo))
                 _lib.check(L.ddnm_conv_tc_bench(N, H, H, Cin, Cout, mode, -iters, C.byref(ms), C.byref(fl)))
                 t[halo].append(ms.value)
-        _lib.check(L.ddnm_tc_debug_halo(1))
+        _lib.check(getattr(L, switch)(1))
         m0, m1 = min(t[0]), min(t[1])
         rows.append(dict(layer=label, ms_off=m0, ms_on=m1, tflops_off=fl.value / m0 / 1e9, tflops_on=fl.value / m1 / 1e9,
                          fill_mb_off=fill_bytes(H, H, Cin, Cout, up2, False) / 1e6, fill_mb_on=fill_bytes(H, H, Cin, Cout, up2, True) / 1e6))
@@ -85,7 +91,7 @@ def bench_shapes(L, iters):
     return rows
 
 
-def forward_profiles(L):
+def forward_profiles(L, switch):
     ns = types.SimpleNamespace
     cfg = ns(model=ns(type="simple", ch=128, out_ch=3, ch_mult=[1, 1, 2, 2, 4, 4], num_res_blocks=2, attn_resolutions=[16], dropout=0.0,
                       in_channels=3, resamp_with_conv=True), data=ns(image_size=256), diffusion=ns(num_diffusion_timesteps=1000))
@@ -95,7 +101,7 @@ def forward_profiles(L):
     t = torch.full((N,), 500.0, device="cuda")
     runs = {0: [], 1: []}
     for halo in (0, 1, 0, 1):
-        _lib.check(L.ddnm_tc_debug_halo(halo))   # read when the engine builds its launches
+        _lib.check(getattr(L, switch)(halo))     # read when the engine builds its launches
         model = Model(cfg)
         model.load_state_dict(sd)
         model.profile(x, t)                      # warm-up: module load, first launches
@@ -103,23 +109,25 @@ def forward_profiles(L):
         model._destroy()
         del model
         torch.cuda.empty_cache()
-    _lib.check(L.ddnm_tc_debug_halo(1))
+    _lib.check(getattr(L, switch)(1))
     return runs
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--switch", choices=sorted(SWITCHES), default="halo")
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
     L = _lib.lib()
-    print("GPU:", gpu_info(), flush=True)
+    switch = SWITCHES[a.switch]
+    print("GPU:", gpu_info(), "| switch:", a.switch, flush=True)
     print(f"\n[1] op-level, N = {N}, pseudo-random operands, best of 2 alternating runs of {a.iters} launches per arm")
     print(f"{'layer':28s} {'ms off':>8s} {'ms on':>8s} {'delta':>7s}  {'TF off':>6s} {'TF on':>6s}  {'fill MB off':>9s} {'fill MB on':>9s}")
-    rows = bench_shapes(L, a.iters)
+    rows = bench_shapes(L, switch, a.iters)
 
     print("\n[2] eager forward, per tensor-core launch (second profile of each engine), arms alternated off/on/off/on")
-    runs = forward_profiles(L)
+    runs = forward_profiles(L, switch)
     tot = {h: [sum(o["ms"] for o in r) for r in runs[h]] for h in runs}
     tc = {h: [sum(o["ms"] for o in r if o["kind"] == "tc") for r in runs[h]] for h in runs}
     best = {h: min(range(2), key=lambda i: tot[h][i]) for h in runs}
@@ -135,7 +143,7 @@ def main():
     print("GPU:", gpu_info(), flush=True)
     if a.json:
         with open(a.json, "w") as f:
-            json.dump(dict(gpu=gpu_info(), shapes=rows, forward=dict(total_ms=tot, tc_ms=tc, off=off, on=on)), f, indent=1)
+            json.dump(dict(gpu=gpu_info(), switch=a.switch, shapes=rows, forward=dict(total_ms=tot, tc_ms=tc, off=off, on=on)), f, indent=1)
 
 
 if __name__ == "__main__":
