@@ -24,6 +24,18 @@ class OpenAICfg(C.Structure):
                 ("eps", C.c_float), ("num_classes", C.c_int)]
 
 
+class ClassifierCfg(C.Structure):
+    _fields_ = [("image_size", C.c_int), ("model_channels", C.c_int), ("num_res_blocks", C.c_int), ("n_levels", C.c_int),
+                ("channel_mult", C.c_int * 8), ("n_attn_ds", C.c_int), ("attn_ds", C.c_int * 4),
+                ("num_head_channels", C.c_int), ("out_channels", C.c_int), ("in_channels", C.c_int), ("groups", C.c_int),
+                ("eps", C.c_float), ("pool", C.c_int)]
+
+
+class ClassifierGuidance(C.Structure):
+    _fields_ = [("classifier", C.c_void_p), ("x", C.c_void_p), ("labels", C.c_void_p), ("scale", C.c_float),
+                ("grad_buf", C.c_void_p), ("batch", C.c_int), ("labels_checked", C.c_int)]
+
+
 class OperatorDesc(C.Structure):
     _fields_ = [("kind", C.c_int), ("channels", C.c_int), ("img_dim", C.c_int), ("ratio", C.c_int),
                 ("v_small", C.c_void_p), ("u_small", C.c_void_p), ("singulars", C.c_void_p),
@@ -56,6 +68,10 @@ _SIGS = {
     "ddnm_version": (C.c_int, []),
     "ddnm_unet_simple_create": (C.c_int, [C.POINTER(SimpleCfg), _I, C.POINTER(_P)]),
     "ddnm_unet_openai_create": (C.c_int, [C.POINTER(OpenAICfg), _I, C.POINTER(_P)]),
+    "ddnm_classifier_create": (C.c_int, [C.POINTER(ClassifierCfg), _I, C.POINTER(_P)]),
+    "ddnm_classifier_forward": (C.c_int, [_P, _P, _P, _P, _P]),
+    "ddnm_classifier_grad": (C.c_int, [_P, _P, _P, _P, _F, _P, _P, _P]),
+    "ddnm_classifier_guidance_fn": (C.c_int, [_P, _I, _I, _P]),
     "ddnm_unet_set_param": (C.c_int, [_P, C.c_char_p, _P, _LL]),
     "ddnm_unet_set_precision": (C.c_int, [_P, _I]),
     "ddnm_unet_finalize": (C.c_int, [_P]),

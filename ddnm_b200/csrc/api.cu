@@ -53,6 +53,59 @@ int ddnm_unet_openai_create(const ddnm_openai_cfg* c, int batch, void** handle) 
   DDNM_API_END
 }
 
+int ddnm_classifier_create(const ddnm_classifier_cfg* c, int batch, void** handle) {
+  DDNM_API_BEGIN
+  DDNM_CHECK(c && handle, "null argument");
+  DDNM_CHECK(c->n_levels >= 1 && c->n_levels <= 8 && c->n_attn_ds >= 0 && c->n_attn_ds <= 4, "bad config");
+  EncoderCfg cfg;
+  cfg.image_size = c->image_size; cfg.model_channels = c->model_channels; cfg.num_res_blocks = c->num_res_blocks;
+  cfg.n_levels = c->n_levels;
+  for (int i = 0; i < 8; ++i) cfg.channel_mult[i] = c->channel_mult[i];
+  cfg.n_attn_ds = c->n_attn_ds;
+  for (int i = 0; i < 4; ++i) cfg.attn_ds[i] = c->attn_ds[i];
+  cfg.num_head_channels = c->num_head_channels; cfg.out_channels = c->out_channels; cfg.in_channels = c->in_channels;
+  cfg.groups = c->groups; cfg.eps = c->eps; cfg.pool = c->pool;
+  *handle = static_cast<UNetEngine*>(new UNetEncoder(cfg, batch));
+  DDNM_API_END
+}
+
+static UNetEncoder* as_classifier(void* h) {
+  UNetEncoder* e = dynamic_cast<UNetEncoder*>(static_cast<UNetEngine*>(h));
+  DDNM_CHECK(e != nullptr, "handle is not a classifier");
+  return e;
+}
+
+int ddnm_classifier_forward(void* h, const float* x, const float* t, float* logits, void* stream) {
+  DDNM_API_BEGIN
+  DDNM_CHECK(x && t && logits, "null argument");
+  as_classifier(h)->forward(x, t, logits, (cudaStream_t)stream);
+  DDNM_API_END
+}
+
+int ddnm_classifier_grad(void* h, const float* x, const float* t, const int* labels, float scale, float* grad_out, float* logits_out,
+                         void* stream) {
+  DDNM_API_BEGIN
+  as_classifier(h)->grad(x, t, labels, scale, grad_out, logits_out, (cudaStream_t)stream);
+  DDNM_API_END
+}
+
+int ddnm_classifier_guidance_fn(void* user, int, int t, void* stream) {
+  DDNM_API_BEGIN
+  ddnm_classifier_guidance* g = static_cast<ddnm_classifier_guidance*>(user);
+  DDNM_CHECK(g && g->classifier && g->x && g->labels && g->grad_buf, "incomplete guidance context");
+  UNetEncoder* e = as_classifier(g->classifier);
+  DDNM_CHECK(g->batch == e->batch(), "classifier was built for batch " + std::to_string(e->batch()) + ", the guided loop runs " +
+                                         std::to_string(g->batch));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!g->labels_checked) {   // the loop's labels are fixed: one host read for the whole loop
+    e->check_labels(g->labels, st);
+    g->labels_checked = 1;
+  }
+  e->fill_t((float)t, st);
+  e->grad(g->x, e->t_in(), g->labels, g->scale, g->grad_buf, nullptr, st, true);
+  DDNM_API_END
+}
+
 int ddnm_unet_set_param(void* h, const char* name, const float* data, long long numel) {
   DDNM_API_BEGIN
   static_cast<UNetEngine*>(h)->set_param(name, data, numel);

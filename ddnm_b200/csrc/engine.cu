@@ -366,8 +366,8 @@ void UNetEngine::finalize() {
   finalized_ = true;
 }
 
-void UNetEngine::run_ops(cudaStream_t s) {
-  for (auto& op : ops_) op.run(s);
+void UNetEngine::run_ops(cudaStream_t s, size_t n) {
+  for (size_t i = 0; i < n && i < ops_.size(); ++i) ops_[i].run(s);
 }
 
 void UNetEngine::set_labels(const int* labels_dev, cudaStream_t stream) {
@@ -379,37 +379,41 @@ void UNetEngine::set_labels(const int* labels_dev, cudaStream_t stream) {
 void UNetEngine::forward(const float* x, const float* t, float* out, cudaStream_t stream) {
   DDNM_CHECK(finalized_, "forward before finalize");
   const size_t xin = (size_t)B_ * in_ch_ * R_ * R_ * 4;
-  const size_t xout = (size_t)B_ * out_ch_ * R_ * R_ * 4;
   if (x != x_in_) CUDA_CHECK(cudaMemcpyAsync(x_in_, x, xin, cudaMemcpyDeviceToDevice, stream));
   if (t != t_in_) CUDA_CHECK(cudaMemcpyAsync(t_in_, t, (size_t)B_ * 4, cudaMemcpyDeviceToDevice, stream));
-  if (use_graph_) {
-    if (!graph_exec_) {
-      // Capture once on a private stream (the caller's may be the legacy default stream, which cannot capture).
-      // A warm-up pass runs first: one-time cudaFuncSetAttribute calls are not capturable.
-      cudaStream_t cs = nullptr;
-      CUDA_CHECK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-      CUDA_CHECK(cudaStreamSynchronize(stream));
-      run_ops(cs);
-      CUDA_CHECK(cudaStreamSynchronize(cs));
-      CUDA_CHECK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
-      try {
-        run_ops(cs);
-      } catch (...) {
-        cudaGraph_t g = nullptr;
-        cudaStreamEndCapture(cs, &g);
-        if (g) cudaGraphDestroy(g);
-        cudaStreamDestroy(cs);
-        throw;
-      }
-      CUDA_CHECK(cudaStreamEndCapture(cs, &graph_));
-      CUDA_CHECK(cudaGraphInstantiate(&graph_exec_, graph_, 0));
-      CUDA_CHECK(cudaStreamDestroy(cs));
-    }
-    CUDA_CHECK(cudaGraphLaunch(graph_exec_, stream));
-  } else {
-    run_ops(stream);
+  replay(stream, ops_.size() - n_tail_ops_, graph_, graph_exec_);
+  if (out != out_) CUDA_CHECK(cudaMemcpyAsync(out, out_, out_elems() * 4, cudaMemcpyDeviceToDevice, stream));
+}
+
+// runs ops_[0, n) on `stream`: eagerly, or as a CUDA graph captured on first use into (g, exec)
+void UNetEngine::replay(cudaStream_t stream, size_t n, cudaGraph_t& g, cudaGraphExec_t& exec) {
+  if (!use_graph_) {
+    run_ops(stream, n);
+    return;
   }
-  if (out != out_) CUDA_CHECK(cudaMemcpyAsync(out, out_, xout, cudaMemcpyDeviceToDevice, stream));
+  if (!exec) {
+    // Capture once on a private stream (the caller's may be the legacy default stream, which cannot capture).
+    // A warm-up pass runs first: one-time cudaFuncSetAttribute calls are not capturable.
+    cudaStream_t cs = nullptr;
+    CUDA_CHECK(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
+    CUDA_CHECK(cudaStreamSynchronize(stream));
+    run_ops(cs, n);
+    CUDA_CHECK(cudaStreamSynchronize(cs));
+    CUDA_CHECK(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
+    try {
+      run_ops(cs, n);
+    } catch (...) {
+      cudaGraph_t gg = nullptr;
+      cudaStreamEndCapture(cs, &gg);
+      if (gg) cudaGraphDestroy(gg);
+      cudaStreamDestroy(cs);
+      throw;
+    }
+    CUDA_CHECK(cudaStreamEndCapture(cs, &g));
+    CUDA_CHECK(cudaGraphInstantiate(&exec, g, 0));
+    CUDA_CHECK(cudaStreamDestroy(cs));
+  }
+  CUDA_CHECK(cudaGraphLaunch(exec, stream));
 }
 
 bool UNetEngine::read_tap(const std::string& name, float* dst, long long capacity, cudaStream_t stream) {

@@ -123,7 +123,10 @@ class UNetEngine {
   void emit_head(const std::string& norm, const std::string& conv, const View& h);
   void alloc_common(size_t split_elems, size_t hbuf_elems);
   virtual void build_program() = 0;
-  void run_ops(cudaStream_t s);
+  // elements of the result forward() copies out: [B, out_ch, R, R] for the denoisers
+  virtual size_t out_elems() const { return (size_t)B_ * out_ch_ * R_ * R_; }
+  void run_ops(cudaStream_t s, size_t n = (size_t)-1);
+  void replay(cudaStream_t stream, size_t n, cudaGraph_t& g, cudaGraphExec_t& exec);
 
   int B_, in_ch_, out_ch_, R_, groups_;
   float eps_;
@@ -133,6 +136,7 @@ class UNetEngine {
   Arena arena_;
   std::map<std::string, Param> params_;
   std::vector<OpRecord> ops_;
+  size_t n_tail_ops_ = 0;   // ops at the end of ops_ that forward() leaves out (the classifier's backward pass)
   std::map<std::string, View> taps_;
   // fixed I/O staging (graph replays need stable addresses)
   float *x_in_ = nullptr, *t_in_ = nullptr, *out_ = nullptr;
@@ -182,6 +186,68 @@ class UNetOpenAI : public UNetEngine {
   int ss_total_ = 0;
   std::map<std::string, int> ss_off_;
   float *embW_all_ = nullptr, *embB_all_ = nullptr;
+};
+
+// guided_diffusion/unet.py::EncoderUNetModel (the classifier of imagenet_256_cc.yml): use_scale_shift_norm, resblock_updown,
+// legacy attention in the blocks, pool "attention" (AttentionPool2d) or "adaptive".  Besides the logits it computes
+//   grad = scale * d/dx sum_b log_softmax(classifier(x, t))[b, labels[b]]       (cond_fn, diffusion.py:183-189)
+// with a hand-written backward pass in the same op list: the forward keeps every GroupNorm input (with its statistics), each
+// attention block's qkv and the head's tokens in dedicated buffers; the convolution data gradients run on the tensor-core
+// kernel with flipped / transposed weights.
+struct EncoderCfg {
+  int image_size = 256, model_channels = 128, num_res_blocks = 2, n_levels = 6;
+  int channel_mult[8] = {1, 1, 2, 2, 4, 4, 0, 0};
+  int n_attn_ds = 3;
+  int attn_ds[4] = {8, 16, 32, 0};
+  int num_head_channels = 64;
+  int out_channels = 1000, in_channels = 3, groups = 32;
+  float eps = 1e-5f;
+  int pool = 1;   // 0 adaptive, 1 attention
+};
+
+class UNetEncoder : public UNetEngine {
+ public:
+  UNetEncoder(const EncoderCfg& cfg, int batch);
+  ~UNetEncoder() override;
+  // logits [B, out_channels] (may be null) and grad [B, in_channels, R, R] (NCHW fp32, device); labels: device int32 [B]
+  // labels_checked: the caller already ran check_labels on these labels (a guided loop checks its fixed labels once)
+  void grad(const float* x, const float* t, const int* labels, float scale, float* grad_out, float* logits, cudaStream_t stream,
+            bool labels_checked = false);
+  // throws unless every label is in [0, out_channels); reads them to the host (synchronises `stream`)
+  void check_labels(const int* labels, cudaStream_t stream) const;
+  // t_in() = t for every image, on the device
+  void fill_t(float t, cudaStream_t stream);
+  int num_classes() const { return cfg_.out_channels; }
+
+ private:
+  void build_program() override;
+  size_t out_elems() const override { return (size_t)B_ * cfg_.out_channels; }
+  struct Res { std::string p; View x, h, out; bool down, skip_conv; };
+  struct Attn { std::string p; View x, out; float* qkv; };
+  struct Layer { int kind; Res r; Attn a; };   // kind 0 ResBlock, 1 AttentionBlock
+  void emit_resblock(const std::string& p, const View& x, const View& out, bool down, Layer& rec);
+  void emit_attn(const std::string& p, const View& x, const View& out, Layer& rec);
+  void emit_head(const View& h);
+  void emit_backward(const View& stem_out, const std::vector<Layer>& layers, const View& top);
+  // GroupNorm (+ scale-shift) (+ SiLU) (+ 2x2 average pool) backward: g = gradient of the block's activation, x = the
+  // GroupNorm input; writes dx (+ add) as fp32 (dx32, may be null) and as the fp16 split `dst` of the next data-gradient convolution
+  void emit_gn_backward(const std::string& name, const float* g, const View& x, const std::string& norm, const float* ss, int ss_ld,
+                        bool silu, bool pool, const float* add, bool add_pool, float* dx32, const SplitView& dst);
+  TcWeights prep_weights_t(const std::string& w, int Cout, int Cin, int taps);
+  EncoderCfg cfg_;
+  float* ss_all_ = nullptr;
+  int ss_total_ = 0;
+  std::map<std::string, int> ss_off_;
+  float *embW_all_ = nullptr, *embB_all_ = nullptr;
+  // head (attention pool): tokens X [B][T][C], qkv [B][T][3C], probabilities [B][heads][T], pooled a0 [B][C]
+  int headT_ = 0;
+  float *hf_ = nullptr, *tok_ = nullptr, *hqkv_ = nullptr, *hp_ = nullptr, *ha0_ = nullptr;
+  // backward scratch
+  float *scale_in_ = nullptr, *grad_ = nullptr, *gx_[2] = {nullptr, nullptr}, *g1_ = nullptr, *g2_ = nullptr, *gqkv_ = nullptr;
+  float *sP_ = nullptr, *sdP_ = nullptr, *gnb_part_ = nullptr;
+  size_t gnb_part_elems_ = 0;
+  cudaGraph_t ggraph_ = nullptr;
+  cudaGraphExec_t ggraph_exec_ = nullptr;
 };
 
 }  // namespace ddnm

@@ -266,3 +266,122 @@ def create_model(image_size, num_channels, num_res_blocks, channel_mult="", lear
                      num_heads=num_heads, num_head_channels=num_head_channels, num_heads_upsample=num_heads_upsample,
                      use_scale_shift_norm=use_scale_shift_norm, resblock_updown=resblock_updown,
                      use_new_attention_order=use_new_attention_order)
+
+
+class EncoderUNetModel(_EngineModel):
+    """guided_diffusion.unet.EncoderUNetModel (unet.py:684-895), the classifier of imagenet_256_cc.yml, for the variant
+    create_classifier builds there (use_scale_shift_norm, resblock_updown, legacy attention order in the blocks, num_head_channels > 0,
+    integer channel multipliers) with pool "attention" or "adaptive".  ``classifier(x, t)`` returns the logits; ``grad(x, t, y, scale)``
+    is the classifier-guidance gradient of diffusion.py:183-189 computed by the library's own backward pass."""
+
+    def __init__(self, image_size, in_channels, model_channels, out_channels, num_res_blocks, attention_resolutions, dropout=0,
+                 channel_mult=(1, 2, 4, 8), conv_resample=True, dims=2, use_checkpoint=False, use_fp16=False, num_heads=1,
+                 num_head_channels=-1, num_heads_upsample=-1, use_scale_shift_norm=False, resblock_updown=False,
+                 use_new_attention_order=False, pool="adaptive"):
+        if pool not in ("adaptive", "attention"):
+            raise NotImplementedError(f"ddnm_b200 EncoderUNetModel: pool {pool!r} is not built (only 'attention' and 'adaptive')")
+        if not (use_scale_shift_norm and resblock_updown) or use_new_attention_order or num_head_channels <= 0 or dims != 2:
+            raise NotImplementedError("ddnm_b200 builds the imagenet_256_cc.yml EncoderUNetModel variant: use_scale_shift_norm, "
+                                      "resblock_updown, legacy attention order, num_head_channels > 0")
+        if any(float(v) != int(v) for v in channel_mult):
+            raise NotImplementedError(f"ddnm_b200 EncoderUNetModel: non-integer channel multipliers {tuple(channel_mult)} are not built")
+        self.image_size = self.resolution = int(image_size)
+        self.in_channels, self.model_channels, self.out_channels = int(in_channels), int(model_channels), int(out_channels)
+        self.out_ch = self.out_channels
+        self.num_res_blocks = int(num_res_blocks)
+        self.attention_resolutions = tuple(int(v) for v in attention_resolutions)
+        self.channel_mult = tuple(int(v) for v in channel_mult)
+        self.num_head_channels = int(num_head_channels)
+        self.pool = pool
+        self.use_fp16 = bool(use_fp16)
+        self.dtype = torch.float32
+        self._init_common()
+
+    def convert_to_fp16(self):
+        """No-op: the reference casts its torso to fp16 here (unet.py:859-864); this engine keeps fp32-grade products
+        on the tensor cores (3x fp16 split), which is at least as accurate as the reference's fp32 mode."""
+        return None
+
+    def convert_to_fp32(self):
+        return None
+
+    def _create(self, batch):
+        c = _lib.ClassifierCfg()
+        c.image_size, c.model_channels, c.num_res_blocks = self.image_size, self.model_channels, self.num_res_blocks
+        c.n_levels = len(self.channel_mult)
+        if not 1 <= c.n_levels <= 8 or len(self.attention_resolutions) > 4:
+            raise NotImplementedError("ddnm_b200 EncoderUNetModel: at most 8 levels and 4 attention resolutions")
+        for i, v in enumerate(self.channel_mult):
+            c.channel_mult[i] = v
+        c.n_attn_ds = len(self.attention_resolutions)
+        for i, v in enumerate(self.attention_resolutions):
+            c.attn_ds[i] = v
+        c.num_head_channels, c.out_channels, c.in_channels, c.groups, c.eps = (self.num_head_channels, self.out_channels,
+                                                                               self.in_channels, 32, 1e-5)
+        c.pool = 1 if self.pool == "attention" else 0
+        h = C.c_void_p()
+        _lib.check(_lib.lib().ddnm_classifier_create(C.byref(c), batch, C.byref(h)))
+        return h
+
+    def _freq(self):
+        half = self.model_channels // 2   # nn.py:113-115
+        return torch.exp(-math.log(10000) * torch.arange(start=0, end=half, dtype=torch.float32) / half)
+
+    def _inputs(self, x, t):
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32):
+            raise _lib.DDNMError("ddnm_b200 classifier runs on CUDA fp32 tensors")
+        if x.dim() != 4 or x.shape[1] != self.in_channels or x.shape[2] != self.image_size or x.shape[3] != self.image_size:
+            raise _lib.DDNMError(f"classifier input must be [B, {self.in_channels}, {self.image_size}, {self.image_size}], got {tuple(x.shape)}")
+        n = x.shape[0]
+        t = torch.as_tensor(t, device=x.device).to(torch.float32).reshape(-1).expand(n).contiguous()
+        return x.contiguous(), t, n
+
+    def forward(self, x, timesteps):
+        x, t, n = self._inputs(x, timesteps)
+        logits = torch.empty(n, self.out_channels, device=x.device, dtype=torch.float32)
+        _lib.check(_lib.lib().ddnm_classifier_forward(self.engine(n), _lib.ptr(x), _lib.ptr(t), _lib.ptr(logits), _lib.cur_stream()))
+        return logits
+
+    def __call__(self, x, timesteps):
+        return self.forward(x, timesteps)
+
+    def profile(self, x, t):
+        """per-op timing of one eager forward + backward (labels 0, scale 1 unless a grad() call set others)"""
+        import json
+        x, t, n = self._inputs(x, t)
+        logits = torch.empty(n, self.out_channels, device=x.device, dtype=torch.float32)
+        buf = C.create_string_buffer(1 << 21)
+        _lib.check(_lib.lib().ddnm_unet_profile(self.engine(n), _lib.ptr(x), _lib.ptr(t), _lib.ptr(logits), _lib.cur_stream(), buf, len(buf)))
+        return json.loads(buf.value.decode())
+
+    def grad(self, x, timesteps, y, scale=1.0, return_logits=False):
+        """scale * d/dx sum_b log_softmax(self(x, t))[b, y_b] (the reference's cond_fn, diffusion.py:183-189)."""
+        x, t, n = self._inputs(x, timesteps)
+        labels = torch.as_tensor(y, device=x.device).reshape(-1).to(torch.int32).contiguous()
+        if labels.numel() != n:
+            raise _lib.DDNMError(f"{labels.numel()} labels for a batch of {n}")
+        g = torch.empty_like(x)
+        logits = torch.empty(n, self.out_channels, device=x.device, dtype=torch.float32) if return_logits else None
+        _lib.check(_lib.lib().ddnm_classifier_grad(self.engine(n), _lib.ptr(x), _lib.ptr(t), _lib.ptr(labels), float(scale), _lib.ptr(g),
+                                                   _lib.ptr(logits), _lib.cur_stream()))
+        return (g, logits) if return_logits else g
+
+
+def create_classifier(image_size, classifier_use_fp16, classifier_width, classifier_depth, classifier_attention_resolutions,
+                      classifier_use_scale_shift_norm, classifier_resblock_updown, classifier_pool):
+    """guided_diffusion.script_util.create_classifier (:229-267), same signature."""
+    if image_size == 512:
+        channel_mult = (0.5, 1, 1, 2, 2, 4, 4)
+    elif image_size == 256:
+        channel_mult = (1, 1, 2, 2, 4, 4)
+    elif image_size == 128:
+        channel_mult = (1, 1, 2, 3, 4)
+    elif image_size == 64:
+        channel_mult = (1, 2, 3, 4)
+    else:
+        raise ValueError(f"unsupported image size: {image_size}")
+    attention_ds = [image_size // int(res) for res in classifier_attention_resolutions.split(",")]
+    return EncoderUNetModel(image_size=image_size, in_channels=3, model_channels=classifier_width, out_channels=1000,
+                            num_res_blocks=classifier_depth, attention_resolutions=tuple(attention_ds), channel_mult=channel_mult,
+                            use_fp16=classifier_use_fp16, num_head_channels=64, use_scale_shift_norm=classifier_use_scale_shift_norm,
+                            resblock_updown=classifier_resblock_updown, pool=classifier_pool)

@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .guidance import ClassifierCondFn
 from .model import _EngineModel
 from .operators import CS, Deblurring2D, GeneralA, SRConv, _Operator
 from .schedule import alpha_bar_table, time_pairs
@@ -110,8 +111,12 @@ def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, n
         if noise is not None and eb != n:
             noise = torch.cat([noise, noise[:, -1:].expand(noise.shape[0], eb - n, *noise.shape[2:])], dim=1).contiguous()
         have_x0 = C.c_int(0)
+        user = None
         if cls_fn is None:
             labels = grad = fn = None
+            failure = []
+        elif isinstance(cls_fn, ClassifierCondFn):
+            labels, grad, fn, user = _native_guidance(x, model, n, cls_fn)
             failure = []
         else:
             labels, grad, fn, failure = _guidance(x, model, n, cls_fn)
@@ -119,7 +124,7 @@ def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, n
         def run_range(k0, k1, chunk):
             rc = _lib.lib().ddnm_sample_range(eng, A_funcs._h, C.byref(s), k0, k1, _lib.ptr(out), _lib.ptr(x0p), C.byref(have_x0),
                                              _lib.ptr(yv), _lib.ptr(chunk), eb, _lib.ptr(labels), _lib.ptr(grad),
-                                             None if fn is None else C.cast(fn, C.c_void_p), None, _lib.cur_stream())
+                                             None if fn is None else C.cast(fn, C.c_void_p), user, _lib.cur_stream())
             if failure:
                 raise failure[0]
             _lib.check(rc)
@@ -160,6 +165,20 @@ def _guidance(x, model, n, cls_fn):
             failure.append(e)
             return 1
     return labels, grad, _lib.GuidanceFn(cb), failure
+
+
+def _native_guidance(x, model, n, cond):
+    """As _guidance, with the gradient computed by the library's classifier (ddnm_classifier_guidance_fn) inside the loop: no
+    host callback.  Returns (labels, grad buffer, C function, guidance context)."""
+    assert model.num_classes is not None, "must specify y if and only if the model is class-conditional"   # unet.py:644-646
+    labels = torch.full((n,), CLASS_NUM, dtype=torch.int32, device=x.device)
+    grad = torch.empty_like(x)
+    ctx = _lib.ClassifierGuidance()
+    ctx.classifier = cond.classifier.engine(n)
+    ctx.x, ctx.labels, ctx.scale, ctx.grad_buf = x.data_ptr(), labels.data_ptr(), cond.scale, grad.data_ptr()
+    ctx.batch, ctx.labels_checked = n, 0
+    # x, labels and grad stay referenced by _run's frame for the whole loop, ctx by the returned pointer
+    return labels, grad, _lib.lib().ddnm_classifier_guidance_fn, C.cast(C.pointer(ctx), C.c_void_p)
 
 
 def ddnm_diffusion(x, model, b, eta, A_funcs, y, cls_fn=None, classes=None, config=None, noise=None):

@@ -141,3 +141,65 @@ def random_state_dict_openai(model, seed=1234, zero_std=0.02):
     for k in zero_keys:
         sd[k] = torch.randn(sd[k].shape, generator=g) * zero_std
     return sd
+
+
+def random_state_dict_classifier(model, seed=1234, zero_std=0.02):
+    """Random-init weights for ``ddnm_b200.model.EncoderUNetModel`` in the reference checkpoint layout, drawn in the layer
+    construction order of unet.py:714-871 after ``torch.manual_seed(seed)``.  As in ``random_state_dict_openai``, the tensors the
+    reference zero-initialises (ResBlock out conv, attention proj_out, the adaptive head's conv) are re-drawn from N(0, zero_std)
+    with generator seed+1: with the reference's own init the input gradient of a random net is degenerate (max |d/dx| ~ 7e-6 at 256^2)."""
+    mc, tdim = model.model_channels, model.model_channels * 4
+    sd, zero_keys = {}, []
+    torch.manual_seed(seed)
+
+    def take(prefix, module, zero=False):
+        for k, v in module.state_dict().items():
+            sd[f"{prefix}.{k}"] = v.detach().clone()
+            if zero:
+                zero_keys.append(f"{prefix}.{k}")
+
+    def res_block(p, cin, cout):
+        take(p + ".in_layers.0", nn.GroupNorm(32, cin))
+        take(p + ".in_layers.2", nn.Conv2d(cin, cout, 3, padding=1))
+        take(p + ".emb_layers.1", nn.Linear(tdim, 2 * cout))
+        take(p + ".out_layers.0", nn.GroupNorm(32, cout))
+        take(p + ".out_layers.3", nn.Conv2d(cout, cout, 3, padding=1), zero=True)
+        if cin != cout:
+            take(p + ".skip_connection", nn.Conv2d(cin, cout, 1))
+
+    def attention(p, c):
+        take(p + ".norm", nn.GroupNorm(32, c))
+        take(p + ".qkv", nn.Conv1d(c, 3 * c, 1))
+        take(p + ".proj_out", nn.Conv1d(c, c, 1), zero=True)
+
+    take("time_embed.0", nn.Linear(mc, tdim))
+    take("time_embed.2", nn.Linear(tdim, tdim))
+    ch = int(model.channel_mult[0] * mc)
+    take("input_blocks.0.0", nn.Conv2d(model.in_channels, ch, 3, padding=1))
+    ds, idx = 1, 1
+    for level, mult in enumerate(model.channel_mult):
+        for _ in range(model.num_res_blocks):
+            res_block(f"input_blocks.{idx}.0", ch, int(mult * mc))
+            ch = int(mult * mc)
+            if ds in model.attention_resolutions:
+                attention(f"input_blocks.{idx}.1", ch)
+            idx += 1
+        if level != len(model.channel_mult) - 1:
+            res_block(f"input_blocks.{idx}.0", ch, ch)
+            idx += 1
+            ds *= 2
+    res_block("middle_block.0", ch, ch)
+    attention("middle_block.1", ch)
+    res_block("middle_block.2", ch, ch)
+    take("out.0", nn.GroupNorm(32, ch))
+    if model.pool == "attention":
+        T = (model.image_size // ds) ** 2 + 1
+        sd["out.2.positional_embedding"] = torch.randn(ch, T) / ch ** 0.5
+        take("out.2.qkv_proj", nn.Conv1d(ch, 3 * ch, 1))
+        take("out.2.c_proj", nn.Conv1d(ch, model.out_channels, 1))
+    else:
+        take("out.3", nn.Conv2d(ch, model.out_channels, 1), zero=True)
+    g = torch.Generator().manual_seed(seed + 1)
+    for k in zero_keys:
+        sd[k] = torch.randn(sd[k].shape, generator=g) * zero_std
+    return sd

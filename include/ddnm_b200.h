@@ -152,6 +152,43 @@ int ddnm_sample_range(void* unet, void* op, const ddnm_schedule* sched, int k_be
                       ddnm_guidance_fn fn, void* user, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Classifier of guided sampling: guided_diffusion/unet.py::EncoderUNetModel (unet.py:684-895) as create_classifier builds it
+ * for imagenet_256_cc.yml (use_scale_shift_norm, resblock_updown, legacy attention, 64-channel heads).  Parameters go through
+ * ddnm_unet_set_param / set_precision / finalize / set_graph / info / profile / destroy with EncoderUNetModel.state_dict() keys
+ * (Conv1d weights keep their (O, I, 1) data) plus "__freq" (the timestep-embedding frequencies).
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  int image_size, model_channels, num_res_blocks, n_levels;
+  int channel_mult[8];
+  int n_attn_ds;
+  int attn_ds[4];             /* downsample rates at which attention runs */
+  int num_head_channels, out_channels, in_channels, groups;
+  float eps;
+  int pool;                   /* 0 = "adaptive", 1 = "attention" */
+} ddnm_classifier_cfg;
+int ddnm_classifier_create(const ddnm_classifier_cfg* cfg, int batch, void** handle);
+/* x [B,3,R,R], t [B] fp32 (device) -> logits [B, out_channels] */
+int ddnm_classifier_forward(void* h, const float* x, const float* t, float* logits, void* stream);
+/* grad_out [B,3,R,R] = scale * d/dx sum_b log_softmax(classifier(x, t))[b, labels[b]]  (cond_fn, diffusion.py:183-189);
+ * labels: device int32 [B], each in [0, out_channels) (checked: the call synchronises `stream` to read them);
+ * logits_out [B, out_channels] may be NULL.  No parameter gradients. */
+int ddnm_classifier_grad(void* h, const float* x, const float* t, const int* labels, float scale, float* grad_out, float* logits_out,
+                         void* stream);
+/* Native classifier guidance for ddnm_sample_guided / ddnm_sample_range: pass ddnm_classifier_guidance_fn as `fn` and a
+ * ddnm_classifier_guidance as `user`; each call leaves the gradient at (x, t) in grad_buf (the loop's grad_buf), with work enqueued on
+ * the loop's stream and no host synchronisation after the first call. */
+typedef struct {
+  void* classifier;           /* ddnm_classifier_create handle built for the sampler's batch */
+  const float* x;             /* device [B,3,R,R]: where the gradient is taken */
+  const int* labels;          /* device int32 [B] */
+  float scale;
+  float* grad_buf;            /* device [B,3,R,R] */
+  int batch;                  /* B of the guided loop: must equal the classifier's batch */
+  int labels_checked;         /* 0 before the loop; set to 1 once the labels were range-checked (then never re-read to the host) */
+} ddnm_classifier_guidance;
+int ddnm_classifier_guidance_fn(void* user, int pair_index, int t, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * "Simplified" DDNM+ (guided_diffusion/diffusion.py:211-415, the README quick-start path): image-space operators composed
  * of mask (A1 = z*mask, :256), colour->gray (color2gray/gray2color, :33-42) and average pooling (AdaptiveAvgPool2d /
  * MeanUpsample, :27-31,:252-253), with the scalar lambda_t / gamma_t update of :355-381.  deg table (:244-290):
