@@ -58,6 +58,10 @@ class Schedule(C.Structure):
                 ("num_timesteps", C.c_int), ("eta", C.c_float), ("sigma_y", C.c_float), ("plus", C.c_int)]
 
 
+class NoiseSeed(C.Structure):
+    _fields_ = [("seed", C.c_ulonglong), ("row_offset", C.c_longlong)]
+
+
 _lib = None
 
 _P, _I, _LL, _F, _D = C.c_void_p, C.c_int, C.c_longlong, C.c_float, C.c_double
@@ -93,6 +97,15 @@ _SIGS = {
     "ddnm_sample": (C.c_int, [_P, _P, C.POINTER(Schedule), _P, _P, _P, _I, _P, _P, _P]),
     "ddnm_sample_guided": (C.c_int, [_P, _P, C.POINTER(Schedule), _P, _P, _P, _I, _P, _P, GuidanceFn, _P, _P, _P, _P]),
     "ddnm_sample_range": (C.c_int, [_P, _P, C.POINTER(Schedule), _I, _I, _P, _P, C.POINTER(C.c_int), _P, _P, _I, _P, _P, _P, _P, _P]),
+    "ddnm_noise_fill": (C.c_int, [C.POINTER(NoiseSeed), C.c_uint, C.c_uint, _P, _I, _LL, _P]),
+    "ddnm_sample_range_seeded": (C.c_int, [_P, _P, C.POINTER(Schedule), _I, _I, _P, _P, C.POINTER(C.c_int), _P, C.POINTER(NoiseSeed), _I,
+                                           _P, _P, _P, _P, _P]),
+    "ddnm_sample_seeded": (C.c_int, [_P, _P, C.POINTER(Schedule), _P, _P, C.POINTER(NoiseSeed), _I, _P, _P, _P]),
+    "ddnm_sample_simplified_range_seeded": (C.c_int, [_P, C.POINTER(SimpleDeg), C.POINTER(Schedule), _I, _I, _P, _P, C.POINTER(C.c_int),
+                                                      _P, C.POINTER(NoiseSeed), _I, _P]),
+    "ddnm_hq_step_seeded": (C.c_int, [C.POINTER(SimpleDeg), _P, _P, _I, _P, _P, _I, _I, _P, _P, C.POINTER(NoiseSeed), C.c_uint,
+                                      C.POINTER(HqScalars), _I, _P, _P, _P, _P]),
+    "ddnm_hq_undo_seeded": (C.c_int, [_P, C.POINTER(NoiseSeed), C.c_uint, _F, _F, _I, _LL, _P]),
     "ddnm_sample_simplified_range": (C.c_int, [_P, C.POINTER(SimpleDeg), C.POINTER(Schedule), _I, _I, _P, _P, C.POINTER(C.c_int), _P, _P,
                                                _I, _P]),
     "ddnm_simplified_A": (C.c_int, [C.POINTER(SimpleDeg), _P, _I, _P, _P]),
@@ -144,6 +157,16 @@ def lib():
 def check(rc):
     if rc != 0:
         raise DDNMError(lib().ddnm_last_error().decode("utf-8", "replace"))
+
+
+def noise_seed(seed, row_offset=0):
+    """ddnm_noise_seed for a 64-bit seed and the global index of the call's first image row."""
+    seed, row_offset = int(seed), int(row_offset)
+    if not 0 <= seed < 1 << 64:
+        raise ValueError("seed must fit 64 unsigned bits")
+    if row_offset < 0:
+        raise ValueError("row_offset must not be negative")
+    return NoiseSeed(seed, row_offset)
 
 
 def ptr(t):

@@ -9,6 +9,7 @@
 #include "../../include/ddnm_b200.h"
 #include "api_util.cuh"
 #include "common.cuh"
+#include "noise.cuh"
 
 namespace ddnm {
 // simplified.cu: A / Ap of the image-space operators on (B, 3, D, D) images
@@ -30,10 +31,12 @@ struct HqRect { int dy, dx, h, w, sy, sx; };   // x0_hat[:, :, dy:dy+h, dx:dx+w]
 
 // x0_hat = lambda*Apy + x0_t - lambda*ApA; mask-shift overwrite; mean = coef1*x0_hat + coef2*x (+ gamma*grad);
 // x_next = mean + nonzero*sqrt(gamma)*noise
+// GEN: the draw is generated in registers from gen, z unused
+template <bool GEN>
 __global__ void hq_combine_kernel(const float* __restrict__ x, const float* __restrict__ x0t, const float* __restrict__ apa,
                                   const float* __restrict__ apy, const float* __restrict__ canvas, int cH, int cW, HqRect r0, HqRect r1,
                                   const float* __restrict__ grad, const float* __restrict__ z, ddnm_hq_scalars s,
-                                  float* __restrict__ x0hat, float* __restrict__ xn, int C, int D, long long n) {
+                                  float* __restrict__ x0hat, float* __restrict__ xn, int C, int D, long long n, NoiseSrc gen) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int px = (int)(i % D), py = (int)((i / D) % D);
@@ -47,13 +50,30 @@ __global__ void hq_combine_kernel(const float* __restrict__ x, const float* __re
   x0hat[i] = v;
   float mean = __fadd_rn(__fmul_rn(s.coef1, v), __fmul_rn(s.coef2, x[i]));
   if (grad) mean = __fadd_rn(mean, __fmul_rn(s.gamma_t, grad[i]));
-  xn[i] = __fadd_rn(mean, __fmul_rn(__fmul_rn(s.nonzero, sqrtf(s.gamma_t)), z[i]));
+  float zi;
+  if (GEN) {
+    const long long b = bc / C;
+    zi = noise_at(gen, (int)b, i - b * C * D * D);
+  } else {
+    zi = z[i];
+  }
+  xn[i] = __fadd_rn(mean, __fmul_rn(__fmul_rn(s.nonzero, sqrtf(s.gamma_t)), zi));
 }
 
 // x = sqrt(1 - beta)*x + sqrt(beta)*noise            (:211-217)
-__global__ void hq_undo_kernel(float* __restrict__ x, const float* __restrict__ z, float a, float b, long long n) {
+template <bool GEN>   // GEN: the draw is generated in registers from gen (img = elements per image), z unused
+__global__ void hq_undo_kernel(float* __restrict__ x, const float* __restrict__ z, float a, float b, long long n, long long img,
+                               NoiseSrc gen) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) x[i] = __fadd_rn(__fmul_rn(a, x[i]), __fmul_rn(b, z[i]));
+  if (i >= n) return;
+  float zi;
+  if (GEN) {
+    const long long r = i / img;
+    zi = noise_at(gen, (int)r, i - r * img);
+  } else {
+    zi = z[i];
+  }
+  x[i] = __fadd_rn(__fmul_rn(a, x[i]), __fmul_rn(b, zi));
 }
 
 // canvas preparation: Apy_temp = Ap(A_temp(gt)) for gt (B, 3, H, W): block means (optionally of the gray image) broadcast back
@@ -83,6 +103,33 @@ __global__ void hq_canvas_kernel(const float* __restrict__ gt, float* __restrict
 }  // namespace ddnm
 
 using namespace ddnm;
+// one mask-shift step with the draw from a tape or generated (ddnm_hq_step / ddnm_hq_step_seeded)
+static void hq_step(const ddnm_simple_deg* deg, const float* x, const float* model_out, int out_ch, const float* apy, const float* canvas,
+                    int canvas_h, int canvas_w, const int* rects, const float* grad, const NoiseSrc& noise, const ddnm_hq_scalars* sc,
+                    int B, float* x0_hat, float* x_next, float* scratch, cudaStream_t st) {
+  DDNM_CHECK(deg && x && model_out && apy && canvas && rects && sc && x0_hat && x_next && scratch, "null argument");
+  DDNM_CHECK(deg->channels == 3 && (out_ch == 3 || out_ch == 6), "hq step: 3-channel images, 3 or 6 model outputs");
+  const int D = deg->img_dim;
+  const long long img = 3LL * D * D, n = (long long)B * img;
+  float* x0t = scratch;          // [n]
+  float* apa = scratch + n;      // [n]
+  float* yb = scratch + 2 * n;   // [<= n]
+  hq_x0_kernel<<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, model_out, (long long)out_ch * D * D, sc->c_recip, sc->c_recipm1, sc->clip, x0t, img, n);
+  simplified_A(deg, x0t, B, yb, st);
+  simplified_Ap(deg, yb, B, apa, st);
+  HqRect r0{rects[0], rects[1], rects[2], rects[3], rects[4], rects[5]}, r1{rects[6], rects[7], rects[8], rects[9], rects[10], rects[11]};
+  for (const HqRect& r : {r0, r1})
+    if (r.h > 0) DDNM_CHECK(r.w > 0 && r.dy >= 0 && r.dx >= 0 && r.dy + r.h <= D && r.dx + r.w <= D && r.sy >= 0 && r.sx >= 0 &&
+                                r.sy + r.h <= canvas_h && r.sx + r.w <= canvas_w, "mask-shift rectangle out of range");
+  if (noise.tape)
+    hq_combine_kernel<false><<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, x0t, apa, apy, canvas, canvas_h, canvas_w, r0, r1, grad, noise.tape,
+                                                                       *sc, x0_hat, x_next, 3, D, n, noise);
+  else
+    hq_combine_kernel<true><<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, x0t, apa, apy, canvas, canvas_h, canvas_w, r0, r1, grad, nullptr,
+                                                                      *sc, x0_hat, x_next, 3, D, n, noise);
+  CUDA_CHECK(cudaGetLastError());
+}
+
 extern "C" {
 int ddnm_hq_canvas(const float* gt, int B, int H, int W, int scale, int use_gray, float* apy_canvas, void* stream) {
   DDNM_API_BEGIN
@@ -97,31 +144,37 @@ int ddnm_hq_step(const ddnm_simple_deg* deg, const float* x, const float* model_
                  int canvas_h, int canvas_w, const int* rects, const float* grad, const float* noise, const ddnm_hq_scalars* sc, int B,
                  float* x0_hat, float* x_next, float* scratch, void* stream) {
   DDNM_API_BEGIN
-  DDNM_CHECK(deg && x && model_out && apy && canvas && rects && noise && sc && x0_hat && x_next && scratch, "null argument");
-  DDNM_CHECK(deg->channels == 3 && (out_ch == 3 || out_ch == 6), "hq step: 3-channel images, 3 or 6 model outputs");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int D = deg->img_dim;
-  const long long img = 3LL * D * D, n = (long long)B * img;
-  float* x0t = scratch;          // [n]
-  float* apa = scratch + n;      // [n]
-  float* yb = scratch + 2 * n;   // [<= n]
-  hq_x0_kernel<<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, model_out, (long long)out_ch * D * D, sc->c_recip, sc->c_recipm1, sc->clip, x0t, img, n);
-  simplified_A(deg, x0t, B, yb, st);
-  simplified_Ap(deg, yb, B, apa, st);
-  HqRect r0{rects[0], rects[1], rects[2], rects[3], rects[4], rects[5]}, r1{rects[6], rects[7], rects[8], rects[9], rects[10], rects[11]};
-  for (const HqRect& r : {r0, r1})
-    if (r.h > 0) DDNM_CHECK(r.w > 0 && r.dy >= 0 && r.dx >= 0 && r.dy + r.h <= D && r.dx + r.w <= D && r.sy >= 0 && r.sx >= 0 &&
-                                r.sy + r.h <= canvas_h && r.sx + r.w <= canvas_w, "mask-shift rectangle out of range");
-  hq_combine_kernel<<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, x0t, apa, apy, canvas, canvas_h, canvas_w, r0, r1, grad, noise, *sc, x0_hat,
-                                                              x_next, 3, D, n);
-  CUDA_CHECK(cudaGetLastError());
+  DDNM_CHECK(noise, "null argument");
+  hq_step(deg, x, model_out, out_ch, apy, canvas, canvas_h, canvas_w, rects, grad, noise_tape(noise), sc, B, x0_hat, x_next, scratch,
+          (cudaStream_t)stream);
+  DDNM_API_END
+}
+int ddnm_hq_step_seeded(const ddnm_simple_deg* deg, const float* x, const float* model_out, int out_ch, const float* apy,
+                        const float* canvas, int canvas_h, int canvas_w, const int* rects, const float* grad,
+                        const ddnm_noise_seed* seed, unsigned draw, const ddnm_hq_scalars* sc, int B, float* x0_hat, float* x_next,
+                        float* scratch, void* stream) {
+  DDNM_API_BEGIN
+  hq_step(deg, x, model_out, out_ch, apy, canvas, canvas_h, canvas_w, rects, grad, noise_seeded(seed, NZ_HQ, draw, B), sc, B, x0_hat,
+          x_next, scratch, (cudaStream_t)stream);
   DDNM_API_END
 }
 
 int ddnm_hq_undo(float* x, const float* noise, float sqrt_one_minus_beta, float sqrt_beta, long long n, void* stream) {
   DDNM_API_BEGIN
   DDNM_CHECK(x && noise && n > 0, "null argument");
-  hq_undo_kernel<<<(unsigned)cdivll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, noise, sqrt_one_minus_beta, sqrt_beta, n);
+  hq_undo_kernel<false><<<(unsigned)cdivll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, noise, sqrt_one_minus_beta, sqrt_beta, n, n,
+                                                                                     NoiseSrc{});
+  CUDA_CHECK(cudaGetLastError());
+  DDNM_API_END
+}
+int ddnm_hq_undo_seeded(float* x, const ddnm_noise_seed* seed, unsigned draw, float sqrt_one_minus_beta, float sqrt_beta, int B,
+                        long long per_image, void* stream) {
+  DDNM_API_BEGIN
+  DDNM_CHECK(x && B >= 1 && per_image > 0, "null argument");
+  const NoiseSrc gen = noise_seeded(seed, NZ_HQ, draw, B);
+  const long long n = (long long)B * per_image;
+  hq_undo_kernel<true><<<(unsigned)cdivll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, nullptr, sqrt_one_minus_beta, sqrt_beta, n,
+                                                                                    per_image, gen);
   CUDA_CHECK(cudaGetLastError());
   DDNM_API_END
 }

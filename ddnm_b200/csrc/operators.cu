@@ -127,12 +127,42 @@ __device__ __forceinline__ float local_resid(const float (&x0)[K], const float* 
   return av;
 }
 
-template <int K, int MODE, int FN>
+// The draws of one group, generated (LF_STEP with a seed).  SuperResolution: a patch row is R consecutive elements starting at
+// a multiple of R, i.e. half a quad (R = 2), one quad (4) or two (8): one Philox call per 2 / 4 values, none wasted.
+// Colorization: the thread owns ONE pixel in three channels, whose values lie in three different quads, so it takes noise_at
+// per value (three Philox calls for three values).  Sharing the quads would need a thread per four pixels, a different kernel
+// from the tape form; at ~1 % of a run's time for all step kernels together that is not worth a second kernel.
+template <int K, int MODE>
+__device__ __forceinline__ void local_draws(const Group<K, MODE>& G, const NoiseSrc& nz, float (&z)[K]) {
+  if (MODE == 0) {
+    constexpr int R = K == 4 ? 2 : (K == 16 ? 4 : 8);
+#pragma unroll
+    for (int kr = 0; kr < R; ++kr) {
+      const long long e = G.base + (long long)kr * G.D;
+      if (R == 2) {
+        const float2 v = noise_pair(nz, G.b, e >> 1);
+        z[kr * R] = v.x; z[kr * R + 1] = v.y;
+      } else {
+#pragma unroll
+        for (int j = 0; j < R / 4; ++j) {
+          const float4 v = noise_quad(nz, G.b, (e >> 2) + j);
+          z[kr * R + 4 * j] = v.x; z[kr * R + 4 * j + 1] = v.y; z[kr * R + 4 * j + 2] = v.z; z[kr * R + 4 * j + 3] = v.w;
+        }
+      }
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < K; ++k) z[k] = noise_at(nz, G.b, G.off(k));
+  }
+}
+
+// GEN (LF_STEP only): in2 is null and the draws are generated in registers from gen
+template <int K, int MODE, int FN, bool GEN = false>
 __global__ void __launch_bounds__(128) local_kernel(const float* __restrict__ in0, const float* __restrict__ in1, long long in1_stride,
                                                     const float* __restrict__ in2, const float* __restrict__ y,
                                                     const float* __restrict__ Vg, float u00, float s0, StepScalars sc,
                                                     float* __restrict__ out0, float* __restrict__ out1, long long groups, int C,
-                                                    int D) {
+                                                    int D, NoiseSrc gen) {
   __shared__ float V[K * K];
   for (int i = threadIdx.x; i < K * K; i += blockDim.x) V[i] = Vg[i];
   __syncthreads();
@@ -200,7 +230,8 @@ __global__ void __launch_bounds__(128) local_kernel(const float* __restrict__ in
     float xt[K], et[K], z[K], x0[K], r[K];
     G.load(in0, img, xt);
     G.load(in1, in1_stride, et);
-    G.load(in2, img, z);
+    if (GEN) local_draws<K, MODE>(G, gen, z);
+    else G.load(in2, img, z);
 #pragma unroll
     for (int k = 0; k < K; ++k) x0[k] = x0_from(xt[k], et[k], sc);
     G.store(out0, img, x0);
@@ -241,16 +272,21 @@ __global__ void __launch_bounds__(128) local_kernel(const float* __restrict__ in
 template <int K, int MODE>
 static void local_launch(int fn, const float* in0, const float* in1, long long in1_stride, const float* in2, const float* y,
                          const float* V, float u00, float s0, const StepScalars& sc, float* out0, float* out1, long long groups,
-                         int C, int D, cudaStream_t st) {
+                         int C, int D, cudaStream_t st, const NoiseSrc* gen = nullptr) {
   const int grid = (int)cdivll(groups, 128);
-#define LL(F) local_kernel<K, MODE, F><<<grid, 128, 0, st>>>(in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D)
+  const NoiseSrc g = gen ? *gen : NoiseSrc{};
+#define LL(F, GEN) \
+  local_kernel<K, MODE, F, GEN><<<grid, 128, 0, st>>>(in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, g)
   switch (fn) {
-    case LF_A: LL(LF_A); break;
-    case LF_PINV: LL(LF_PINV); break;
-    case LF_PROJECT: LL(LF_PROJECT); break;
-    case LF_LAMBDA: LL(LF_LAMBDA); break;
-    case LF_NOISE: LL(LF_NOISE); break;
-    default: LL(LF_STEP); break;
+    case LF_A: LL(LF_A, false); break;
+    case LF_PINV: LL(LF_PINV, false); break;
+    case LF_PROJECT: LL(LF_PROJECT, false); break;
+    case LF_LAMBDA: LL(LF_LAMBDA, false); break;
+    case LF_NOISE: LL(LF_NOISE, false); break;
+    default:
+      if (gen) LL(LF_STEP, true);
+      else LL(LF_STEP, false);
+      break;
   }
 #undef LL
   CUDA_CHECK(cudaGetLastError());
@@ -260,10 +296,11 @@ static void local_launch(int fn, const float* in0, const float* in1, long long i
 // Inpainting (svd_operators.py:324-439; mask -> indices at diffusion.py:464-471).  y holds the kept entries of the
 // (pixel, channel)-interleaved image in ascending order: y[rank(p*C + c)] = x[c][p].  Pure data movement: bit-exact.
 // ------------------------------------------------------------------------------------------------------------------
-template <int FN>
+template <int FN, bool GEN = false>   // GEN (LF_STEP only): draws generated in registers from gen, in2 unused
 __global__ void inpaint_kernel(const float* __restrict__ in0, const float* __restrict__ in1, long long in1_stride,
                                const float* __restrict__ in2, const float* __restrict__ y, const int* __restrict__ rank,
-                               StepScalars sc, float* __restrict__ out0, float* __restrict__ out1, int B, int C, int HW, long long M) {
+                               StepScalars sc, float* __restrict__ out0, float* __restrict__ out1, int B, int C, int HW, long long M,
+                               NoiseSrc gen) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long img = (long long)C * HW;
   if (i >= (long long)B * img) return;
@@ -290,7 +327,7 @@ __global__ void inpaint_kernel(const float* __restrict__ in0, const float* __res
     out0[i] = __fadd_rn(__fmul_rn(in0[i], d1), __fmul_rn(in1[(long long)b * in1_stride + (i - (long long)b * img)], d2));
   } else {
     const float et = in1[(long long)b * in1_stride + (i - (long long)b * img)];
-    const float z = in2[i];
+    const float z = GEN ? noise_at(gen, b, i - (long long)b * img) : in2[i];
     const float x0 = x0_from(in0[i], et, sc);
     out0[i] = x0;
     const float resid = kept ? __fsub_rn(x0, y[yi]) : 0.f;
@@ -404,11 +441,20 @@ __global__ void x0_kernel(const float* __restrict__ xt, const float* __restrict_
   et3[i] = e;
   x0[i] = x0_from(xt[i], e, sc);
 }
+template <bool GEN>   // GEN: draws generated in registers from gen (img = elements per image), z unused
 __global__ void final_ddnm_kernel(const float* __restrict__ x0, const float* __restrict__ resid, const float* __restrict__ z,
-                                  const float* __restrict__ et3, StepScalars sc, float* __restrict__ xn, long long n) {
+                                  const float* __restrict__ et3, StepScalars sc, float* __restrict__ xn, long long n, long long img,
+                                  NoiseSrc gen) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  xn[i] = renoise(__fsub_rn(x0[i], resid[i]), z[i], et3[i], sc);
+  float zi;
+  if (GEN) {
+    const long long b = i / img;
+    zi = noise_at(gen, (int)b, i - b * img);
+  } else {
+    zi = z[i];
+  }
+  xn[i] = renoise(__fsub_rn(x0[i], resid[i]), zi, et3[i], sc);
 }
 __global__ void final_plus_kernel(const float* __restrict__ x0, const float* __restrict__ L, const float* __restrict__ nz,
                                   StepScalars sc, float* __restrict__ xn, long long n) {
@@ -461,10 +507,10 @@ __global__ void cs_patch_kernel(const float* __restrict__ src, float* __restrict
 }
 
 // Denoising (svd_operators.py:442-476): A = I; Lambda / Lambda_noise are SCALAR rules of their own (not the table rule)
-template <int FN>
+template <int FN, bool GEN = false>   // GEN (LF_STEP only): draws generated in registers from gen, in2 unused
 __global__ void denoise_kernel(const float* __restrict__ in0, const float* __restrict__ in1, long long in1_stride,
                                const float* __restrict__ in2, const float* __restrict__ y, StepScalars sc, float* __restrict__ out0,
-                               float* __restrict__ out1, int B, long long img) {
+                               float* __restrict__ out1, int B, long long img, NoiseSrc gen) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)B * img) return;
   const int b = (int)(i / img);
@@ -480,7 +526,7 @@ __global__ void denoise_kernel(const float* __restrict__ in0, const float* __res
     out0[i] = (ps.sigma_t >= asy) ? __fmul_rn(in0[i], sqrtf(t2)) : __fmul_rn(__fmul_rn(in0[i], ps.sigma_t), ps.eta);
   } else {  // LF_STEP
     const float et = in1[(long long)b * in1_stride + (i - (long long)b * img)];
-    const float z = in2[i];
+    const float z = GEN ? noise_at(gen, b, i - (long long)b * img) : in2[i];
     const float x0 = x0_from(in0[i], et, sc);
     out0[i] = x0;
     const float resid = __fsub_rn(x0, y[i]);
@@ -690,14 +736,14 @@ static inline int blocks(long long n, int t = 256) { return (int)cdivll(n, t); }
 template <int FN>
 static void local_dispatch(int kind, int ratio, const float* in0, const float* in1, long long in1_stride, const float* in2,
                            const float* y, const float* V, float u00, float s0, const StepScalars& sc, float* out0, float* out1,
-                           int B, int C, int D, cudaStream_t st) {
+                           int B, int C, int D, cudaStream_t st, const NoiseSrc* gen = nullptr) {
   if (kind == OP_COLOR) {
-    local_launch<3, 1>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, (long long)B * D * D, C, D, st);
+    local_launch<3, 1>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, (long long)B * D * D, C, D, st, gen);
   } else {
     const long long groups = (long long)B * C * (D / ratio) * (D / ratio);
-    if (ratio == 2) local_launch<4, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st);
-    else if (ratio == 4) local_launch<16, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st);
-    else local_launch<64, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st);
+    if (ratio == 2) local_launch<4, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, gen);
+    else if (ratio == 4) local_launch<16, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, gen);
+    else local_launch<64, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, gen);
   }
 }
 
@@ -950,7 +996,7 @@ void Operator::A(const float* x, int B, float* y, cudaStream_t s) {
       local_dispatch<LF_A>(kind_, ratio_, x, nullptr, 0, nullptr, nullptr, V_, u00_, s0_, sc, y, nullptr, B, C_, D_, s);
       break;
     case OP_INPAINT:
-      inpaint_kernel<LF_A><<<blocks((long long)B * C_ * n2), 256, 0, s>>>(x, nullptr, 0, nullptr, nullptr, rank_, sc, y, nullptr, B, C_, n2, M_);
+      inpaint_kernel<LF_A><<<blocks((long long)B * C_ * n2), 256, 0, s>>>(x, nullptr, 0, nullptr, nullptr, rank_, sc, y, nullptr, B, C_, n2, M_, NoiseSrc{});
       break;
     case OP_WH: {
       const long long n = (long long)B * C_ * n2;
@@ -987,7 +1033,7 @@ void Operator::A_pinv(const float* y, int B, float* x, cudaStream_t s) {
       local_dispatch<LF_PINV>(kind_, ratio_, nullptr, nullptr, 0, nullptr, y, V_, u00_, s0_, sc, x, nullptr, B, C_, D_, s);
       break;
     case OP_INPAINT:
-      inpaint_kernel<LF_PINV><<<blocks((long long)B * C_ * n2), 256, 0, s>>>(nullptr, nullptr, 0, nullptr, y, rank_, sc, x, nullptr, B, C_, n2, M_);
+      inpaint_kernel<LF_PINV><<<blocks((long long)B * C_ * n2), 256, 0, s>>>(nullptr, nullptr, 0, nullptr, y, rank_, sc, x, nullptr, B, C_, n2, M_, NoiseSrc{});
       break;
     case OP_WH:
       wh_spec_kernel<LF_PINV><<<blocks((long long)B * C_ * n2), 256, 0, s>>>(nullptr, nullptr, y, perm_, invperm_, sc.plus, x, B, C_, n2, M_);
@@ -1019,7 +1065,7 @@ void Operator::project(const float* x0, const float* y, int B, float* out, cudaS
       local_dispatch<LF_PROJECT>(kind_, ratio_, x0, nullptr, 0, nullptr, y, V_, u00_, s0_, sc, out, nullptr, B, C_, D_, s);
       break;
     case OP_INPAINT:
-      inpaint_kernel<LF_PROJECT><<<blocks(n), 256, 0, s>>>(x0, nullptr, 0, nullptr, y, rank_, sc, out, nullptr, B, C_, n2, M_);
+      inpaint_kernel<LF_PROJECT><<<blocks(n), 256, 0, s>>>(x0, nullptr, 0, nullptr, y, rank_, sc, out, nullptr, B, C_, n2, M_, NoiseSrc{});
       break;
     case OP_WH: {
       float* F = scratch(0, n);
@@ -1049,7 +1095,7 @@ void Operator::lambda(const float* v, int B, const PlusScalars& ps, float* out, 
   const int n2 = D_ * D_;
   const long long n = (long long)B * C_ * n2;
   if (kind_ == OP_DENOISE) {
-    denoise_kernel<LF_LAMBDA><<<blocks(n), 256, 0, s>>>(v, nullptr, 0, nullptr, nullptr, sc, out, nullptr, B, (long long)C_ * n2);
+    denoise_kernel<LF_LAMBDA><<<blocks(n), 256, 0, s>>>(v, nullptr, 0, nullptr, nullptr, sc, out, nullptr, B, (long long)C_ * n2, NoiseSrc{});
     CUDA_CHECK(cudaGetLastError());
     return;
   }
@@ -1066,7 +1112,7 @@ void Operator::lambda(const float* v, int B, const PlusScalars& ps, float* out, 
       local_dispatch<LF_LAMBDA>(kind_, ratio_, v, nullptr, 0, nullptr, nullptr, V_, u00_, s0_, sc, out, nullptr, B, C_, D_, s);
       break;
     case OP_INPAINT:
-      inpaint_kernel<LF_LAMBDA><<<blocks(n), 256, 0, s>>>(v, nullptr, 0, nullptr, nullptr, rank_, sc, out, nullptr, B, C_, n2, M_);
+      inpaint_kernel<LF_LAMBDA><<<blocks(n), 256, 0, s>>>(v, nullptr, 0, nullptr, nullptr, rank_, sc, out, nullptr, B, C_, n2, M_, NoiseSrc{});
       break;
     case OP_WH: {
       float* F = scratch(0, n);
@@ -1097,7 +1143,7 @@ void Operator::lambda_noise(const float* v, const float* eps, int B, const PlusS
   const long long n = (long long)B * C_ * n2;
   const long long img = (long long)C_ * n2;
   if (kind_ == OP_DENOISE) {
-    denoise_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, nullptr, 0, nullptr, nullptr, sc, out, nullptr, B, img);
+    denoise_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, nullptr, 0, nullptr, nullptr, sc, out, nullptr, B, img, NoiseSrc{});
     CUDA_CHECK(cudaGetLastError());
     return;
   }
@@ -1114,7 +1160,7 @@ void Operator::lambda_noise(const float* v, const float* eps, int B, const PlusS
       local_dispatch<LF_NOISE>(kind_, ratio_, v, eps, img, nullptr, nullptr, V_, u00_, s0_, sc, out, nullptr, B, C_, D_, s);
       break;
     case OP_INPAINT:
-      inpaint_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, eps, img, nullptr, nullptr, rank_, sc, out, nullptr, B, C_, n2, M_);
+      inpaint_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, eps, img, nullptr, nullptr, rank_, sc, out, nullptr, B, C_, n2, M_, NoiseSrc{});
       break;
     case OP_WH:
       wh_spec_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, eps, nullptr, perm_, invperm_, ps, out, B, C_, n2, M_);
@@ -1133,17 +1179,22 @@ void Operator::lambda_noise(const float* v, const float* eps, int B, const PlusS
   CUDA_CHECK(cudaGetLastError());
 }
 
-void Operator::step(const float* xt, const float* et, long long et_stride, const float* noise, const float* y, int B,
+void Operator::step(const float* xt, const float* et, long long et_stride, const NoiseSrc& nz, const float* y, int B,
                     const StepScalars& sc, float* x0_t, float* xt_next, cudaStream_t s) {
   const int n2 = D_ * D_;
   const long long img = N_;
   const long long n = (long long)B * img;
+  const float* noise = nz.tape;
+  const bool gen = noise == nullptr;
   if ((kind_ == OP_SR && !sr_generic_) || kind_ == OP_COLOR) {
-    local_dispatch<LF_STEP>(kind_, ratio_, xt, et, et_stride, noise, y, V_, u00_, s0_, sc, x0_t, xt_next, B, C_, D_, s);
+    local_dispatch<LF_STEP>(kind_, ratio_, xt, et, et_stride, noise, y, V_, u00_, s0_, sc, x0_t, xt_next, B, C_, D_, s,
+                            gen ? &nz : nullptr);
   } else if (kind_ == OP_INPAINT) {
-    inpaint_kernel<LF_STEP><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, rank_, sc, x0_t, xt_next, B, C_, n2, M_);
+    if (gen) inpaint_kernel<LF_STEP, true><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, nullptr, y, rank_, sc, x0_t, xt_next, B, C_, n2, M_, nz);
+    else inpaint_kernel<LF_STEP><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, rank_, sc, x0_t, xt_next, B, C_, n2, M_, nz);
   } else if (kind_ == OP_DENOISE) {
-    denoise_kernel<LF_STEP><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, sc, x0_t, xt_next, B, img);
+    if (gen) denoise_kernel<LF_STEP, true><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, nullptr, y, sc, x0_t, xt_next, B, img, nz);
+    else denoise_kernel<LF_STEP><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, sc, x0_t, xt_next, B, img, nz);
   } else {
     // generic path: x0_t, residual r = A^+(A x0_t - y), then the DDNM / DDNM+ update
     float* et3 = scratch(5, n);
@@ -1168,8 +1219,16 @@ void Operator::step(const float* xt, const float* et, long long et_stride, const
       }
     }
     if (!sc.use_plus) {
-      final_ddnm_kernel<<<blocks(n), 256, 0, s>>>(x0_t, R, noise, et3, sc, xt_next, n);
+      if (gen) final_ddnm_kernel<true><<<blocks(n), 256, 0, s>>>(x0_t, R, nullptr, et3, sc, xt_next, n, img, nz);
+      else final_ddnm_kernel<false><<<blocks(n), 256, 0, s>>>(x0_t, R, noise, et3, sc, xt_next, n, img, nz);
     } else {
+      if (gen) {
+        // Lambda_noise of these operators is a transform of the whole draw (a GEMM or a Walsh-Hadamard transform of the raw
+        // pixels), not a map: materialise this ONE pair's draws, the same values the fused kernels make in registers
+        float* Z = scratch(10, (size_t)n);
+        noise_fill(nz, Z, B, img, s);
+        noise = Z;
+      }
       lambda(R, B, sc.plus, R, s);                       // R <- Lambda(R)   (in place is safe: inputs are staged first)
       float* NZ = scratch(3, std::max<size_t>((size_t)n, (size_t)B * M_));
       lambda_noise(noise, et3, B, sc.plus, NZ, s);

@@ -4,6 +4,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "noise.cuh"
 
 namespace ddnm {
 
@@ -41,7 +42,9 @@ class Operator {
   void lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s);
   // One sampler step: x0_t = (xt - et*sqrt(1-at))/sqrt(at); x0_hat by projection (and Lambda); xt_next.
   // et_stride = elements between consecutive images of et (6-channel nets keep channels 0..2).
-  void step(const float* xt, const float* et, long long et_stride, const float* noise, const float* y, int B, const StepScalars& sc,
+  // noise: a tape of this pair's draws, or a generated source (noise.cuh): the fused kernels then produce the values in
+  // registers, and the operators whose Lambda_noise is a transform fill one pair's worth of scratch first.
+  void step(const float* xt, const float* et, long long et_stride, const NoiseSrc& noise, const float* y, int B, const StepScalars& sc,
             float* x0_t, float* xt_next, cudaStream_t s);
   static PlusScalars make_plus(float a, float sigma_y, float sigma_t, float eta);
 
@@ -76,8 +79,8 @@ class Operator {
   int *rank_ = nullptr;      // inpaint: kept-rank per pixel or -1
   int *perm_ = nullptr, *invperm_ = nullptr;
   std::vector<void*> owned_;
-  float* scr_[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  size_t scr_elems_[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  float* scr_[11] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  size_t scr_elems_[11] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // [10]: one pair of generated draws (step, seeded DDNM+)
 };
 
 }  // namespace ddnm

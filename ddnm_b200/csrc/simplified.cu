@@ -7,6 +7,7 @@
 #include "../../include/ddnm_b200.h"
 #include "api_util.cuh"
 #include "engine.cuh"
+#include "noise.cuh"
 
 namespace ddnm {
 
@@ -21,10 +22,12 @@ struct SimpDeg {
 enum { SF_A = 0, SF_AP = 1, SF_STEP = 2 };
 
 // A(z) = pool(gray(z * mask)),  Ap(v) = gray2color(upsample(v)) * mask   (whichever stages are enabled)
-template <int S, int FN>
+// GEN (SF_STEP only): the draws are generated in registers from gen, z unused.  A patch row is S consecutive elements starting
+// at a multiple of S, so one generator call serves min(S, 4) values: noise_at (S = 1), noise_pair (2), noise_quad (4, 8).
+template <int S, int FN, bool GEN = false>
 __global__ void __launch_bounds__(128) simp_kernel(const float* __restrict__ in0, const float* __restrict__ et, long long et_stride,
                                                    const float* __restrict__ z, const float* __restrict__ y, SimpDeg dg, SimpScalars sc,
-                                                   float* __restrict__ out0, float* __restrict__ out1, int B) {
+                                                   float* __restrict__ out0, float* __restrict__ out1, int B, NoiseSrc gen) {
   constexpr int K = S * S;
   const int D = dg.D, yd = D / S;
   const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -93,6 +96,8 @@ __global__ void __launch_bounds__(128) simp_kernel(const float* __restrict__ in0
   float r[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) r[c] = __fsub_rn(a[c], y[yo + (long long)c * yd * yd]);
+  constexpr int W = S >= 4 ? 4 : S;   // values per generator call
+  float zg[4];
 #pragma unroll
   for (int c = 0; c < 3; ++c)
 #pragma unroll
@@ -101,7 +106,18 @@ __global__ void __launch_bounds__(128) simp_kernel(const float* __restrict__ in0
       if (dg.use_mask) w = __fmul_rn(w, m[k]);
       const float x0h = __fsub_rn(x0[c][k], __fmul_rn(sc.lambda_t, w));                       // Eq. 17 (:373)
       const float e = et[(long long)b * et_stride + off(c, k)];
-      const float zz = z[(long long)b * img + off(c, k)];
+      if (GEN && k % W == 0) {
+        if (W == 4) {
+          const float4 v = noise_quad(gen, b, off(c, k) >> 2);
+          zg[0] = v.x; zg[1] = v.y; zg[2] = v.z; zg[3] = v.w;
+        } else if (W == 2) {
+          const float2 v = noise_pair(gen, b, off(c, k) >> 1);
+          zg[0] = v.x; zg[1] = v.y;
+        } else {
+          zg[0] = noise_at(gen, b, off(c, k));
+        }
+      }
+      const float zz = GEN ? zg[k % W] : z[(long long)b * img + off(c, k)];
       const float nz = __fmul_rn(sc.gamma_t, __fadd_rn(__fmul_rn(sc.c1, zz), __fmul_rn(sc.c2, e)));  // (:381)
       out1[(long long)b * img + off(c, k)] = __fadd_rn(__fmul_rn(sc.sqrt_atn, x0h), nz);
     }
@@ -109,10 +125,11 @@ __global__ void __launch_bounds__(128) simp_kernel(const float* __restrict__ in0
 
 // Any other scale (evaluation.sh runs sr_averagepooling with deg_scale 16): one WARP per patch, lanes stride over the S*S pixels,
 // the three channel sums meet through shuffles.  Same arithmetic per element as simp_kernel; the pooled sums are re-associated.
-template <int FN>
+template <int FN, bool GEN = false>   // GEN (SF_STEP only): noise_at per value (a lane's pixels are 32 apart), z unused
 __global__ void __launch_bounds__(128) simp_generic_kernel(const float* __restrict__ in0, const float* __restrict__ et, long long et_stride,
                                                            const float* __restrict__ z, const float* __restrict__ y, SimpDeg dg,
-                                                           SimpScalars sc, float* __restrict__ out0, float* __restrict__ out1, int B) {
+                                                           SimpScalars sc, float* __restrict__ out0, float* __restrict__ out1, int B,
+                                                           NoiseSrc gen) {
   const int S = dg.scale, K = S * S;
   const int D = dg.D, yd = D / S;
   const long long g = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -188,26 +205,26 @@ __global__ void __launch_bounds__(128) simp_generic_kernel(const float* __restri
       const float x0 = out0[(long long)b * img + o];                                            // written above by this thread
       const float x0h = __fsub_rn(x0, __fmul_rn(sc.lambda_t, w));                               // Eq. 17 (:373)
       const float e = et[(long long)b * et_stride + o];
-      const float zz = z[(long long)b * img + o];
+      const float zz = GEN ? noise_at(gen, b, o) : z[(long long)b * img + o];
       const float nz = __fmul_rn(sc.gamma_t, __fadd_rn(__fmul_rn(sc.c1, zz), __fmul_rn(sc.c2, e)));  // (:381)
       out1[(long long)b * img + o] = __fadd_rn(__fmul_rn(sc.sqrt_atn, x0h), nz);
     }
   }
 }
 
-template <int FN>
+template <int FN, bool GEN = false>
 static void simp_launch(const SimpDeg& dg, const float* in0, const float* et, long long et_stride, const float* z, const float* y,
-                        const SimpScalars& sc, float* out0, float* out1, int B, cudaStream_t st) {
+                        const SimpScalars& sc, float* out0, float* out1, int B, cudaStream_t st, const NoiseSrc& gen = NoiseSrc{}) {
   const int yd = dg.D / dg.scale;
   const long long groups = (long long)B * yd * yd;
   const int grid = (int)cdivll(groups, 128);
   switch (dg.scale) {
-    case 1: simp_kernel<1, FN><<<grid, 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B); break;
-    case 2: simp_kernel<2, FN><<<grid, 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B); break;
-    case 4: simp_kernel<4, FN><<<grid, 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B); break;
-    case 8: simp_kernel<8, FN><<<grid, 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B); break;
+    case 1: simp_kernel<1, FN, GEN><<<grid, 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B, gen); break;
+    case 2: simp_kernel<2, FN, GEN><<<grid, 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B, gen); break;
+    case 4: simp_kernel<4, FN, GEN><<<grid, 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B, gen); break;
+    case 8: simp_kernel<8, FN, GEN><<<grid, 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B, gen); break;
     default:   // any other scale dividing the image size
-      simp_generic_kernel<FN><<<(int)cdivll(groups * 32, 128), 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B);
+      simp_generic_kernel<FN, GEN><<<(int)cdivll(groups * 32, 128), 128, 0, st>>>(in0, et, et_stride, z, y, dg, sc, out0, out1, B, gen);
   }
   CUDA_CHECK(cudaGetLastError());
 }
@@ -225,16 +242,25 @@ __global__ void simp_fill_kernel(float* p, int n, float v) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
 }
+template <bool GEN>   // GEN: the draw is generated in registers from gen (img = elements per image), z unused
 __global__ void simp_travel_kernel(const float* __restrict__ x0, const float* __restrict__ z, float sa, float s1, float* __restrict__ xn,
-                                   long long n) {
+                                   long long n, long long img, NoiseSrc gen) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) xn[i] = __fadd_rn(__fmul_rn(sa, x0[i]), __fmul_rn(z[i], s1));
+  if (i >= n) return;
+  float zi;
+  if (GEN) {
+    const long long b = i / img;
+    zi = noise_at(gen, (int)b, i - b * img);
+  } else {
+    zi = z[i];
+  }
+  xn[i] = __fadd_rn(__fmul_rn(sa, x0[i]), __fmul_rn(zi, s1));
 }
 
 // pairs [k0, k1) with the state in the caller's buffers (same contract as sample_range in sampler.cu)
 static void sample_simplified_range(UNetEngine* unet, const ddnm_simple_deg* d, const ddnm_schedule* sc, int k0, int k1, float* xt_state,
-                                    float* x0t, int* have_x0, const float* y, const float* noise, int B, cudaStream_t st) {
-  DDNM_CHECK(unet && sc && xt_state && x0t && have_x0 && y && noise, "null argument");
+                                    float* x0t, int* have_x0, const float* y, const NoiseSrc& noise, int B, cudaStream_t st) {
+  DDNM_CHECK(unet && sc && xt_state && x0t && have_x0 && y, "null argument");
   DDNM_CHECK(unet->batch() == B, "engine was built for a different batch size");
   DDNM_CHECK(0 <= k0 && k0 <= k1 && k1 <= sc->n_pairs, "pair range outside the schedule");
   SimpDeg dg = make_deg(d);
@@ -253,7 +279,9 @@ static void sample_simplified_range(UNetEngine* unet, const ddnm_simple_deg* d, 
     const int i = sc->t_i[k], j = sc->t_j[k];
     DDNM_CHECK(i >= 0 && i < sc->num_timesteps && j >= -1 && j < sc->num_timesteps, "time index out of range");
     const float at_next = sc->abar[j + 1];
-    const float* z = noise + (long long)(k - k0) * n;
+    NoiseSrc z = noise;   // a tape holds the draws of exactly these pairs; a generated source is indexed by the pair
+    if (z.tape) z.tape += (long long)(k - k0) * n;
+    else z.draw = (unsigned)k;
     if (j < i) {
       const float at = sc->abar[i + 1];
       simp_fill_kernel<<<cdiv(B, 128), 128, 0, st>>>(unet->t_in(), B, (float)i);
@@ -275,11 +303,14 @@ static void sample_simplified_range(UNetEngine* unet, const ddnm_simple_deg* d, 
         s.lambda_t = sigma_t / asy;
         s.gamma_t = 0.0f;
       }
-      simp_launch<SF_STEP>(dg, xt, et, et_stride, z, y, s, x0t, xn, B, st);
+      if (z.tape) simp_launch<SF_STEP>(dg, xt, et, et_stride, z.tape, y, s, x0t, xn, B, st);
+      else simp_launch<SF_STEP, true>(dg, xt, et, et_stride, nullptr, y, s, x0t, xn, B, st, z);
       *have_x0 = 1;
     } else {
       DDNM_CHECK(*have_x0, "schedule starts with a travel-back step");
-      simp_travel_kernel<<<(int)cdivll(n, 256), 256, 0, st>>>(x0t, z, std::sqrt(at_next), std::sqrt(1.0f - at_next), xn, n);
+      const float sa = std::sqrt(at_next), s1 = std::sqrt(1.0f - at_next);
+      if (z.tape) simp_travel_kernel<false><<<(int)cdivll(n, 256), 256, 0, st>>>(x0t, z.tape, sa, s1, xn, n, 3LL * R * R, z);
+      else simp_travel_kernel<true><<<(int)cdivll(n, 256), 256, 0, st>>>(x0t, nullptr, sa, s1, xn, n, 3LL * R * R, z);
       CUDA_CHECK(cudaGetLastError());
     }
     CUDA_CHECK(cudaMemcpyAsync(xt, xn, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -300,7 +331,7 @@ static void sample_simplified(UNetEngine* unet, const ddnm_simple_deg* d, const 
   }
   if (out_x0 != x_T) CUDA_CHECK(cudaMemcpyAsync(out_x0, x_T, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
   int have_x0 = 0;
-  sample_simplified_range(unet, d, sc, 0, sc->n_pairs, out_x0, x0t, &have_x0, y, noise, B, st);
+  sample_simplified_range(unet, d, sc, 0, sc->n_pairs, out_x0, x0t, &have_x0, y, noise_tape(noise), B, st);
 }
 
 // used by the hq_demo mask-shift step (hq.cu)
@@ -332,8 +363,17 @@ int ddnm_simplified_Ap(const ddnm_simple_deg* d, const float* y, int B, float* x
 int ddnm_sample_simplified_range(void* unet, const ddnm_simple_deg* d, const ddnm_schedule* sched, int k_begin, int k_end, float* xt,
                                  float* x0_pred, int* have_x0, const float* y, const float* noise, int B, void* stream) {
   DDNM_API_BEGIN
-  sample_simplified_range(static_cast<UNetEngine*>(unet), d, sched, k_begin, k_end, xt, x0_pred, have_x0, y, noise, B,
+  DDNM_CHECK(noise, "null argument");
+  sample_simplified_range(static_cast<UNetEngine*>(unet), d, sched, k_begin, k_end, xt, x0_pred, have_x0, y, noise_tape(noise), B,
                           (cudaStream_t)stream);
+  DDNM_API_END
+}
+int ddnm_sample_simplified_range_seeded(void* unet, const ddnm_simple_deg* d, const ddnm_schedule* sched, int k_begin, int k_end,
+                                        float* xt, float* x0_pred, int* have_x0, const float* y, const ddnm_noise_seed* seed, int B,
+                                        void* stream) {
+  DDNM_API_BEGIN
+  sample_simplified_range(static_cast<UNetEngine*>(unet), d, sched, k_begin, k_end, xt, x0_pred, have_x0, y,
+                          noise_seeded(seed, NZ_LOOP, 0, B), B, (cudaStream_t)stream);
   DDNM_API_END
 }
 int ddnm_sample_simplified(void* unet, const ddnm_simple_deg* d, const ddnm_schedule* sched, const float* x_T, const float* y,

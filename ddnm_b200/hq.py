@@ -20,6 +20,7 @@ import torch
 
 from . import _lib
 from .model import _EngineModel
+from .noise import TAG_HQ, randn
 
 
 def get_schedule_jump(t_T, n_sample, jump_length, jump_n_sample, jump2_length=1, jump2_n_sample=1, jump3_length=1, jump3_n_sample=1,
@@ -138,11 +139,14 @@ def _shift_rects(sh, sw, sh_total, sw_total, H, W):
 
 
 def restore(model, gt, classes, deg="sr_averagepooling", scale=4, sigma_y=0.0, resize_y=False, timestep_respacing=100,
-            schedule_jump_params=None, diffusion_steps=1000, clip_denoised=True, cond_fn=None, noise=None):
+            schedule_jump_params=None, diffusion_steps=1000, clip_denoised=True, cond_fn=None, noise=None, seed=None):
     """gt: the degraded input image(s) (B,3,h,w) in [-1,1] on the GPU (main.py:103-110); returns the restored canvas as a CPU
     tensor (B,3,H,W) — H, W = gt's size (x scale with ``resize_y``).  ``noise``: optional (n_draws,B,3,256,256) tape in the
     reference's draw order (initial x, then one per p_sample / undo call); by default the draws come from torch's generator in
-    that order."""
+    that order.  ``seed``: the library draws them instead (stream tag 3, draw index = position in that order, row = image), inside
+    the step kernels; reproducible against itself, not against torch's generator."""
+    if seed is not None and noise is not None:
+        raise ValueError("seed= and noise= are two sources for the same draws: give one")
     if not isinstance(model, _EngineModel):
         model = getattr(model, "module", model)
     if not isinstance(model, _EngineModel) or model.num_classes is None or model.out_ch != 6 or model.resolution != 256:
@@ -175,13 +179,20 @@ def restore(model, gt, classes, deg="sr_averagepooling", scale=4, sigma_y=0.0, r
         d.use_mask, d.use_gray, d.scale, d.img_dim, d.channels, d.mask = 0, use_gray, sc, 256, 3, None
         labels = torch.as_tensor(classes).to(dev).long().reshape(-1)
         tape = None if noise is None else noise.to(dev).float().contiguous()
+        ns = None if seed is None else _lib.noise_seed(seed)
         draws = [0]
 
         def draw():
+            """The next draw: a tensor (torch / tape modes), or its index (seeded mode: the kernels generate the values)."""
             k = draws[0]
             draws[0] += 1
+            if ns is not None:
+                return k
             return torch.randn(B, 3, 256, 256, device=dev) if tape is None else tape[k]
-        x = draw().clone()                                      # th.randn(*shape) (:574); carried over from window to window
+        if ns is None:
+            x = draw().clone()                                  # th.randn(*shape) (:574); carried over from window to window
+        else:
+            x = randn(seed, (B, 3, 256, 256), TAG_HQ, draw=draw(), device=dev)
         x_next, x0_hat = torch.empty_like(x), torch.empty_like(x)
         scratch = torch.empty(3 * x.numel(), device=dev)
         times = get_schedule_jump(**jump)
@@ -214,14 +225,22 @@ def restore(model, gt, classes, deg="sr_averagepooling", scale=4, sigma_y=0.0, r
                                 grad = cond_fn(x, torch.full((B,), K.timestep_map[t], device=dev, dtype=torch.long), labels)
                             grad = grad.float().contiguous()
                         z = draw()
-                        _lib.check(L.ddnm_hq_step(C.byref(d), _lib.ptr(x), _lib.ptr(mo), 6, _lib.ptr(apy), _lib.ptr(final), H, W, rects,
-                                                  _lib.ptr(grad), _lib.ptr(z), C.byref(s), B, _lib.ptr(x0_hat), _lib.ptr(x_next),
-                                                  _lib.ptr(scratch), _lib.cur_stream()))
+                        if ns is None:
+                            _lib.check(L.ddnm_hq_step(C.byref(d), _lib.ptr(x), _lib.ptr(mo), 6, _lib.ptr(apy), _lib.ptr(final), H, W, rects,
+                                                      _lib.ptr(grad), _lib.ptr(z), C.byref(s), B, _lib.ptr(x0_hat), _lib.ptr(x_next),
+                                                      _lib.ptr(scratch), _lib.cur_stream()))
+                        else:
+                            _lib.check(L.ddnm_hq_step_seeded(C.byref(d), _lib.ptr(x), _lib.ptr(mo), 6, _lib.ptr(apy), _lib.ptr(final), H, W,
+                                                             rects, _lib.ptr(grad), C.byref(ns), z, C.byref(s), B, _lib.ptr(x0_hat),
+                                                             _lib.ptr(x_next), _lib.ptr(scratch), _lib.cur_stream()))
                         x, x_next = x_next, x
                     else:
                         beta = np.float32(K.betas[t_last + 1])              # inpa_inj_time_shift = 1 (:727-733)
                         z = draw()
-                        _lib.check(L.ddnm_hq_undo(_lib.ptr(x), _lib.ptr(z), float(np.sqrt(np.float32(1.0) - beta, dtype=np.float32)),
-                                                  float(np.sqrt(beta, dtype=np.float32)), x.numel(), _lib.cur_stream()))
+                        a, bb = float(np.sqrt(np.float32(1.0) - beta, dtype=np.float32)), float(np.sqrt(beta, dtype=np.float32))
+                        if ns is None:
+                            _lib.check(L.ddnm_hq_undo(_lib.ptr(x), _lib.ptr(z), a, bb, x.numel(), _lib.cur_stream()))
+                        else:
+                            _lib.check(L.ddnm_hq_undo_seeded(_lib.ptr(x), C.byref(ns), z, a, bb, B, x[0].numel(), _lib.cur_stream()))
                 final[:, :, h_l:h_l + 256, w_l:w_l + 256] = x0_hat           # :737-747
         return final.to("cpu")

@@ -24,6 +24,23 @@ def sharded_sample(sample_fn, x, y, noise=None, group=None):
     lo, hi = shard_rows(B, rank, world)
     nz = None if noise is None else noise[:, lo:hi]
     x0, x0p = sample_fn(x[lo:hi], y[lo:hi], nz)
+    return _gather_rows(x0, x0p, B, lo, hi, world, group)
+
+
+def sharded_sample_seeded(sample_fn, x, y, seed, group=None):
+    """As ``sharded_sample`` with library-drawn noise: runs ``sample_fn(x_rows, y_rows, seed, row_offset=lo)`` on this rank's rows
+    [lo, hi) and all-gathers.  A seeded draw depends on the GLOBAL row index only, so no rank needs a noise tape and the result
+    equals the unsharded ``sample_fn(x, y, seed, row_offset=0)`` row for row, at any world size."""
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    rank = dist.get_rank(group) if dist.is_initialized() else 0
+    B = x.shape[0]
+    lo, hi = shard_rows(B, rank, world)
+    x0, x0p = sample_fn(x[lo:hi], y[lo:hi], seed, row_offset=lo)
+    return _gather_rows(x0, x0p, B, lo, hi, world, group)
+
+
+def _gather_rows(x0, x0p, B, lo, hi, world, group):
+    """All ranks' (x0, x0_pred) row blocks -> the full batch on every rank."""
     if world == 1:
         return x0, x0p
     counts = [shard_rows(B, r, world) for r in range(world)]

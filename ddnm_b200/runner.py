@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .noise import TAG_XT, TAG_Y, randn
 from .sampler import sample_device
 
 
@@ -128,13 +129,17 @@ def _save_all(folder, pattern, u8_cuda, idx0):
 
 
 def restore_batch(config, model, A_funcs, deg, x_orig, betas, eta, sigma_y=0.0, add_noise=False, image_folder=None, idx_so_far=0,
-                  x_T=None, noise=None, cls_fn=None):
+                  x_T=None, noise=None, cls_fn=None, seed=None):
     """Body of the reference's evaluation loop for one batch (guided_diffusion/diffusion.py:533-603).
 
     x_orig: (B,C,H,W) in [0,1] (what the DataLoader yields), host or CUDA.  ``sigma_y`` is the level the reference passes on,
     i.e. already doubled (diffusion.py:524).  Returns a dict with ``psnr`` (B,) CPU, ``images`` (B,H,W,C) uint8 numpy,
     ``Apy`` / ``orig`` previews (uint8 numpy) and ``y``; PNGs are written under ``image_folder`` with the reference's names
     when it is given.
+
+    ``seed``: x_T, the ``add_noise`` term and the loop's draws come from the library's seeded generator with
+    ``row_offset = idx_so_far``, so image i of a dataset restores identically whatever ``sampling.batch_size`` is (the
+    dequantisation draws of ``data_transform``, off in every shipped config, stay torch's).
     """
     dev = torch.device("cuda")
     C_, R = config.data.channels, config.data.image_size
@@ -142,7 +147,9 @@ def restore_batch(config, model, A_funcs, deg, x_orig, betas, eta, sigma_y=0.0, 
         x_orig = data_transform(config, x_orig.to(dev, non_blocking=True))                # :534-535
         y = A_funcs.A(x_orig)                                                             # :537
         b, hwc = y.shape
-        if add_noise:                                                                     # :550-551 (same draw count and order)
+        if add_noise and seed is not None:
+            y = y + randn(seed, y.shape, TAG_Y, row_offset=idx_so_far, device=dev) * sigma_y
+        elif add_noise:                                                                   # :550-551 (same draw count and order)
             y = get_gaussian_noisy_img(y, sigma_y)
         Apy = A_funcs.A_pinv(y).view(b, C_, R, R)                                         # :555
         if deg[:6] == "deblur":                                                           # :558-560
@@ -153,11 +160,14 @@ def restore_batch(config, model, A_funcs, deg, x_orig, betas, eta, sigma_y=0.0, 
             Apy = Apy + (A_funcs.A_pinv(A_funcs.A(torch.ones_like(Apy))).reshape(*Apy.shape) - 1)
         apy_u8, _, _ = finish_images(config, Apy)
         orig_u8, _, _ = finish_images(config, x_orig)
-        if x_T is None:
+        if x_T is None and seed is not None:
+            x_T = randn(seed, (b, C_, R, R), TAG_XT, row_offset=idx_so_far, device=dev)
+        elif x_T is None:
             x_T = torch.randn(b, C_, R, R, device=dev)                                    # :578-584
         plus = sigma_y != 0.0                                                             # :587-590
         x0, _ = sample_device(x_T, model, betas, eta, A_funcs, y, sigma_y if plus else 0.0, plus, config, noise=noise,
-                              cls_fn=cls_fn)                                              # cls_fn: diffusion.py:181-189 (class-conditional configs)
+                              cls_fn=cls_fn, seed=seed,                                # cls_fn: diffusion.py:181-189 (class-conditional configs)
+                              row_offset=idx_so_far if seed is not None else 0)
         img_u8, psnr, _ = finish_images(config, x0, x_orig)                               # :592-601
         out = dict(psnr=psnr.cpu(), y=y)
         if image_folder is not None:

@@ -5,6 +5,11 @@ The whole loop runs inside libddnm_b200.so on the current CUDA stream without ho
 are taken from torch's generator in the reference's order (one ``randn_like`` per time pair, :65/:74), a bounded chunk of
 pairs at a time on a side stream while the previous chunk is being denoised (``NOISE_CHUNK_BYTES``), so a run is
 seed-for-seed comparable with the reference on the same device and its noise memory does not grow with the schedule.
+
+With ``seed=`` the library draws the Gaussians itself (include/ddnm_b200.h, "Seeded noise"): a value is a pure function of
+(seed, global image row, pair index, element), generated inside the step kernels, so the loop is one library call with no
+noise memory, and image ``row_offset + b`` restores identically whatever batch, padding or rank it ran in.  Those draws are
+not torch's: a seeded run is reproducible against itself, not seed-for-seed against the reference.
 """
 import ctypes as C
 
@@ -70,12 +75,25 @@ def _chunked(n_pairs, x, run_range, rows=None):
         b.record_stream(side)                               # allocated on the caller's stream, written on the side stream
 
 
-def sample_device(x, model, b, eta, A_funcs, y, sigma_y, plus, config, noise=None, cls_fn=None):
+def sample_device(x, model, b, eta, A_funcs, y, sigma_y, plus, config, noise=None, cls_fn=None, seed=None, row_offset=0):
     """The loop with device-resident inputs and outputs (no host copies): returns (x_0, x0_pred) CUDA tensors."""
-    return _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, None, config, noise, to_host=False)
+    return _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, None, config, noise, to_host=False, seed=seed,
+                row_offset=row_offset)
 
 
-def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, noise=None, to_host=True):
+def _noise_mode(noise, seed, row_offset):
+    """The ddnm_noise_seed of a seeded run, or None for the tape / torch-drawn modes."""
+    if seed is None:
+        if row_offset != 0:
+            raise ValueError("row_offset only applies to seeded noise (seed=...)")
+        return None
+    if noise is not None:
+        raise ValueError("seed= and noise= are two sources for the same draws: give one")
+    return _lib.noise_seed(seed, row_offset)
+
+
+def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, noise=None, to_host=True, seed=None, row_offset=0):
+    ns = _noise_mode(noise, seed, row_offset)
     if not isinstance(model, _EngineModel):
         model = getattr(model, "module", model)          # tolerate nn.DataParallel-style wrappers
     if not isinstance(model, _EngineModel) or not isinstance(A_funcs, _Operator):
@@ -128,7 +146,15 @@ def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, n
             if failure:
                 raise failure[0]
             _lib.check(rc)
-        if noise is not None:
+        if ns is not None:
+            # one call over the whole schedule; the rows a ragged batch was padded with are just further image rows
+            rc = _lib.lib().ddnm_sample_range_seeded(eng, A_funcs._h, C.byref(s), 0, len(pairs), _lib.ptr(out), _lib.ptr(x0p),
+                                                    C.byref(have_x0), _lib.ptr(yv), C.byref(ns), eb, _lib.ptr(labels), _lib.ptr(grad),
+                                                    None if fn is None else C.cast(fn, C.c_void_p), user, _lib.cur_stream())
+            if failure:
+                raise failure[0]
+            _lib.check(rc)
+        elif noise is not None:
             run_range(0, len(pairs), noise)
         else:
             _chunked(len(pairs), x, run_range, rows=eb)
@@ -181,12 +207,13 @@ def _native_guidance(x, model, n, cond):
     return labels, grad, _lib.lib().ddnm_classifier_guidance_fn, C.cast(C.pointer(ctx), C.c_void_p)
 
 
-def ddnm_diffusion(x, model, b, eta, A_funcs, y, cls_fn=None, classes=None, config=None, noise=None):
-    return _run(x, model, b, eta, A_funcs, y, 0.0, False, cls_fn, classes, config, noise)
+def ddnm_diffusion(x, model, b, eta, A_funcs, y, cls_fn=None, classes=None, config=None, noise=None, seed=None, row_offset=0):
+    return _run(x, model, b, eta, A_funcs, y, 0.0, False, cls_fn, classes, config, noise, seed=seed, row_offset=row_offset)
 
 
-def ddnm_plus_diffusion(x, model, b, eta, A_funcs, y, sigma_y, cls_fn=None, classes=None, config=None, noise=None):
-    return _run(x, model, b, eta, A_funcs, y, sigma_y, True, cls_fn, classes, config, noise)
+def ddnm_plus_diffusion(x, model, b, eta, A_funcs, y, sigma_y, cls_fn=None, classes=None, config=None, noise=None, seed=None,
+                        row_offset=0):
+    return _run(x, model, b, eta, A_funcs, y, sigma_y, True, cls_fn, classes, config, noise, seed=seed, row_offset=row_offset)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -228,9 +255,11 @@ class SimplifiedDegradation:
         return x
 
 
-def simplified_ddnm_plus(x, model, b, eta, degradation, y, sigma_y, config=None, noise=None):
+def simplified_ddnm_plus(x, model, b, eta, degradation, y, sigma_y, config=None, noise=None, seed=None, row_offset=0):
     """x: x_T (B,3,H,W); y = degradation.A(x_orig); sigma_y already doubled (diffusion.py:292).  Returns
-    ``([x_0.cpu()], [x0_pred.cpu()])`` like the SVD samplers."""
+    ``([x_0.cpu()], [x0_pred.cpu()])`` like the SVD samplers.  ``seed`` / ``row_offset``: library-drawn noise, as in
+    ``ddnm_diffusion``."""
+    ns = _noise_mode(noise, seed, row_offset)
     if not isinstance(model, _EngineModel):
         model = getattr(model, "module", model)
     if not isinstance(model, _EngineModel) or not isinstance(degradation, SimplifiedDegradation):
@@ -259,7 +288,11 @@ def simplified_ddnm_plus(x, model, b, eta, degradation, y, sigma_y, config=None,
             _lib.check(_lib.lib().ddnm_sample_simplified_range(eng, C.byref(degradation._d), C.byref(s), k0, k1, _lib.ptr(out),
                                                               _lib.ptr(x0p), C.byref(have_x0), _lib.ptr(yv), _lib.ptr(chunk), n,
                                                               _lib.cur_stream()))
-        if noise is not None:
+        if ns is not None:
+            _lib.check(_lib.lib().ddnm_sample_simplified_range_seeded(eng, C.byref(degradation._d), C.byref(s), 0, len(pairs),
+                                                                     _lib.ptr(out), _lib.ptr(x0p), C.byref(have_x0), _lib.ptr(yv),
+                                                                     C.byref(ns), n, _lib.cur_stream()))
+        elif noise is not None:
             run_range(0, len(pairs), noise)
         else:
             _chunked(len(pairs), x, run_range)

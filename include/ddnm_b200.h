@@ -152,6 +152,31 @@ int ddnm_sample_range(void* unet, void* op, const ddnm_schedule* sched, int k_be
                       ddnm_guidance_fn fn, void* user, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Seeded noise: the library draws the Gaussians itself, no tape and no caller-side generator.  The value of one element is a
+ * pure function of (seed, stream tag, global image row, draw index, element index): Philox4x32-10 with key = (seed low 32,
+ * seed high 32) and counter = (element / 4, draw, row_offset + local row, tag); the four outputs become the normals of elements
+ * 4q .. 4q+3 through u = ((x >> 9) + 0.5) * 2^-23 and Box-Muller on (x0,x1), (x2,x3): sqrtf(-2 logf(u_a)) * {cospif, sinpif}(2 u_b).
+ * Batch size, padding, the cut of a schedule into ranges and the number of GPUs do not enter, so image `row` of a dataset
+ * restores identically however the work is split.  tags: 0 = the loop's draws (draw = pair index), 1 = x_T, 2 = measurement
+ * noise on y, 3 = hq_demo's draws (draw = position in its draw order), 4 = dequantisation noise.
+ * These streams are NOT torch's: runs that must be seed-for-seed comparable with the reference keep using the tape entries.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+  unsigned long long seed;
+  long long row_offset;       /* global index of this call's first image row (>= 0) */
+} ddnm_noise_seed;
+/* out [B, per_image] (16-byte aligned when per_image % 4 == 0) = the draws of (tag, draw) for rows row_offset .. row_offset+B-1 */
+int ddnm_noise_fill(const ddnm_noise_seed* seed, unsigned tag, unsigned draw, float* out, int B, long long per_image, void* stream);
+/* ddnm_sample_range with generated draws (tag 0, draw = pair index, whatever [k_begin, k_end) is).  The fused step kernels
+ * produce the values in registers; operators whose Lambda_noise is a transform fill one pair's worth of scratch owned by `op`. */
+int ddnm_sample_range_seeded(void* unet, void* op, const ddnm_schedule* sched, int k_begin, int k_end, float* xt, float* x0_pred,
+                             int* have_x0, const float* y, const ddnm_noise_seed* seed, int B, const int* labels,
+                             const float* grad_buf, ddnm_guidance_fn fn, void* user, void* stream);
+/* The whole unguided loop in one call; x_T may be NULL: it is then generated too (tag 1, draw 0). */
+int ddnm_sample_seeded(void* unet, void* op, const ddnm_schedule* sched, const float* x_T, const float* y, const ddnm_noise_seed* seed,
+                       int B, float* out_x0, float* out_x0_pred, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Classifier of guided sampling: guided_diffusion/unet.py::EncoderUNetModel (unet.py:684-895) as create_classifier builds it
  * for imagenet_256_cc.yml (use_scale_shift_norm, resblock_updown, legacy attention, 64-channel heads).  Parameters go through
  * ddnm_unet_set_param / set_precision / finalize / set_graph / info / profile / destroy with EncoderUNetModel.state_dict() keys
@@ -208,6 +233,10 @@ int ddnm_sample_simplified(void* unet, const ddnm_simple_deg* deg, const ddnm_sc
 /* pairs [k_begin, k_end) with caller-held state: same contract as ddnm_sample_range */
 int ddnm_sample_simplified_range(void* unet, const ddnm_simple_deg* deg, const ddnm_schedule* sched, int k_begin, int k_end, float* xt,
                                  float* x0_pred, int* have_x0, const float* y, const float* noise, int B, void* stream);
+/* the same with generated draws (tag 0, draw = pair index) */
+int ddnm_sample_simplified_range_seeded(void* unet, const ddnm_simple_deg* deg, const ddnm_schedule* sched, int k_begin, int k_end,
+                                        float* xt, float* x0_pred, int* have_x0, const float* y, const ddnm_noise_seed* seed, int B,
+                                        void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * hq_demo: arbitrary-size restoration with the mask-shift trick (hq_demo/guided_diffusion/gaussian_diffusion.py:318-390 "DDNM core",
@@ -232,6 +261,13 @@ int ddnm_hq_step(const ddnm_simple_deg* deg, const float* x, const float* model_
                  int canvas_h, int canvas_w, const int* rects, const float* grad, const float* noise, const ddnm_hq_scalars* sc, int B,
                  float* x0_hat, float* x_next, float* scratch, void* stream);
 int ddnm_hq_undo(float* x, const float* noise, float sqrt_one_minus_beta, float sqrt_beta, long long n, void* stream);
+/* the same two with generated draws (tag 3); `draw` = position of this draw in the host loop's draw order */
+int ddnm_hq_step_seeded(const ddnm_simple_deg* deg, const float* x, const float* model_out, int out_ch, const float* apy,
+                        const float* canvas, int canvas_h, int canvas_w, const int* rects, const float* grad,
+                        const ddnm_noise_seed* seed, unsigned draw, const ddnm_hq_scalars* sc, int B, float* x0_hat, float* x_next,
+                        float* scratch, void* stream);
+int ddnm_hq_undo_seeded(float* x, const ddnm_noise_seed* seed, unsigned draw, float sqrt_one_minus_beta, float sqrt_beta, int B,
+                        long long per_image, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * The runner's I/O step either side of the loop (guided_diffusion/diffusion.py:533-603), device pointers throughout.
