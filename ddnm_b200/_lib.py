@@ -21,7 +21,7 @@ class OpenAICfg(C.Structure):
     _fields_ = [("image_size", C.c_int), ("model_channels", C.c_int), ("num_res_blocks", C.c_int), ("n_levels", C.c_int),
                 ("channel_mult", C.c_int * 8), ("n_attn_ds", C.c_int), ("attn_ds", C.c_int * 4),
                 ("num_head_channels", C.c_int), ("out_channels", C.c_int), ("in_channels", C.c_int), ("groups", C.c_int),
-                ("eps", C.c_float), ("num_classes", C.c_int)]
+                ("eps", C.c_float), ("num_classes", C.c_int), ("low_res", C.c_int)]
 
 
 class ClassifierCfg(C.Structure):
@@ -82,6 +82,7 @@ _SIGS = {
     "ddnm_unet_forward": (C.c_int, [_P, _P, _P, _P, _P]),
     "ddnm_unet_forward_cond": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "ddnm_unet_set_graph": (C.c_int, [_P, _I]),
+    "ddnm_unet_set_low_res": (C.c_int, [_P, _P, _P]),
     "ddnm_unet_read_tap": (C.c_int, [_P, C.c_char_p, _P, _LL, _P]),
     "ddnm_unet_info": (C.c_int, [_P, C.POINTER(_LL), C.POINTER(_I), C.POINTER(_D)]),
     "ddnm_unet_profile": (C.c_int, [_P, _P, _P, _P, _P, C.c_char_p, _LL]),
@@ -119,6 +120,7 @@ _SIGS = {
     "ddnm_finish_images": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
     "ddnm_conv_tc": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P]),
     "ddnm_conv_direct": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P]),
+    "ddnm_conv_stem_sr": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _P, _I, C.POINTER(_F), _P]),
     "ddnm_conv_tc_bench": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, C.POINTER(_F), C.POINTER(_D)]),
     "ddnm_gnconv_chunk_bench": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, C.POINTER(_F)]),
     "ddnm_groupnorm": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, _F, _I, _P, _P]),

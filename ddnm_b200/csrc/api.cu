@@ -47,7 +47,7 @@ int ddnm_unet_openai_create(const ddnm_openai_cfg* c, int batch, void** handle) 
   cfg.n_attn_ds = c->n_attn_ds;
   for (int i = 0; i < 4; ++i) cfg.attn_ds[i] = c->attn_ds[i];
   cfg.num_head_channels = c->num_head_channels; cfg.out_channels = c->out_channels; cfg.in_channels = c->in_channels;
-  cfg.groups = c->groups; cfg.eps = c->eps; cfg.num_classes = c->num_classes;
+  cfg.groups = c->groups; cfg.eps = c->eps; cfg.num_classes = c->num_classes; cfg.low_res = c->low_res;
   DDNM_CHECK(c->num_classes >= 0, "bad num_classes");
   *handle = static_cast<UNetEngine*>(new UNetOpenAI(cfg, batch));
   DDNM_API_END
@@ -126,6 +126,11 @@ int ddnm_unet_forward_cond(void* h, const float* x, const float* t, const int* l
   UNetEngine* u = static_cast<UNetEngine*>(h);
   u->set_labels(labels, (cudaStream_t)stream);
   u->forward(x, t, out, (cudaStream_t)stream);
+  DDNM_API_END
+}
+int ddnm_unet_set_low_res(void* h, const float* low_res, void* stream) {
+  DDNM_API_BEGIN
+  static_cast<UNetEngine*>(h)->set_low_res(low_res, (cudaStream_t)stream);
   DDNM_API_END
 }
 int ddnm_unet_set_precision(void* h, int fp16_terms) {
@@ -242,6 +247,33 @@ int ddnm_conv_tc(const float* x, int N, int H, int W, int Cin, const float* w, c
   if (side_x) split_conv_weight(side_w, Cout, CinSide, 1, wh, wl, ktot, taps * Cin, s);
   TcLaunch L = tc_make_launch(A, mode, side_x ? &S : nullptr, wh, wl, 1, Cout, ov, bias, 0, residual, Cout, 1.0f, sm_count());
   tc_run(L, s);
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  DDNM_API_END
+}
+
+// the super-resolution stem on its own: out (NHWC [N,H,W,Cout]) = conv3x3(cat([x, bilinear(low_res)])) + bias; low_res == NULL:
+// x is the already concatenated [N,2C,H,W] (the composed form).  iters > 0: also time `iters` launches.
+int ddnm_conv_stem_sr(const float* x, const float* low_res, int N, int C, int H, int W, int h, int w, const float* weight,
+                      const float* bias, int Cout, float* out, int iters, float* ms_per_iter, void* stream) {
+  DDNM_API_BEGIN
+  DDNM_CHECK(x && weight && bias && out, "null argument");
+  cudaStream_t s = (cudaStream_t)stream;
+  View ov = mkview(out, N, H, W, Cout);
+  conv3x3_stem_sr(x, low_res, C, h, w, weight, bias, ov, s);
+  if (iters > 0 && ms_per_iter) {
+    cudaEvent_t e0, e1;
+    CUDA_CHECK(cudaEventCreate(&e0));
+    CUDA_CHECK(cudaEventCreate(&e1));
+    CUDA_CHECK(cudaEventRecord(e0, s));
+    for (int i = 0; i < iters; ++i) conv3x3_stem_sr(x, low_res, C, h, w, weight, bias, ov, s);
+    CUDA_CHECK(cudaEventRecord(e1, s));
+    CUDA_CHECK(cudaEventSynchronize(e1));
+    float ms = 0;
+    CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    *ms_per_iter = ms / iters;
+  }
   CUDA_CHECK(cudaStreamSynchronize(s));
   DDNM_API_END
 }

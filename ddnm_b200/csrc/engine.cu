@@ -217,6 +217,7 @@ void UNetEngine::alloc_common(size_t split_elems, size_t hbuf_elems) {
   labels_in_ = (int*)arena_.alloc((size_t)B_ * 4);
   CUDA_CHECK(cudaMemset(labels_in_, 0, (size_t)B_ * 4));
   out_ = (float*)arena_.alloc((size_t)B_ * out_ch_ * R_ * R_ * 4);
+  if (lowres_ > 0) lowres_in_ = (float*)arena_.alloc((size_t)B_ * in_ch_ * lowres_ * lowres_ * 4);
 }
 
 void UNetEngine::emit_up2_conv(const std::string& name, const SplitView& a, const std::string& wname, int Cout, const View& out,
@@ -286,9 +287,19 @@ void UNetEngine::emit_attention_core(const std::string& name, int T, int heads, 
   }
 }
 
-// network stem: 3x3 conv on the caller's NCHW tensor -> NHWC view
+// network stem: 3x3 conv on the caller's NCHW tensor -> NHWC view.  Super-resolution networks convolve cat([x, bilinear(low_res)])
+// (2 * in_ch_ input channels) with the upsampled half computed inside the kernel from the staged low_res.
 void UNetEngine::emit_stem(const std::string& wname, const View& out) {
   const float* xin = x_in_;
+  if (lowres_ > 0) {
+    const float *w = P(wname + ".weight", (long long)out.C * 2 * in_ch_ * 9), *b = P(wname + ".bias", out.C);
+    const float* lr = lowres_in_;
+    const int cin = in_ch_, s = lowres_;
+    add_op("stem.sr", "stem", 2.0 * B_ * R_ * R_ * (double)out.C * 2 * cin * 9,
+           (double)B_ * (R_ * R_ * (cin + out.C) + (double)s * s * cin) * 4,
+           [=](cudaStream_t st) { conv3x3_stem_sr(xin, lr, cin, s, s, w, b, out, st); });
+    return;
+  }
   const float *w = P(wname + ".weight", (long long)out.C * in_ch_ * 9), *b = P(wname + ".bias", out.C);
   const int cin = in_ch_;
   add_op("stem", "stem", 2.0 * B_ * R_ * R_ * (double)out.C * cin * 9, (double)B_ * R_ * R_ * (cin + out.C) * 4,
@@ -376,8 +387,17 @@ void UNetEngine::set_labels(const int* labels_dev, cudaStream_t stream) {
   if (labels_dev != labels_in_) CUDA_CHECK(cudaMemcpyAsync(labels_in_, labels_dev, (size_t)B_ * sizeof(int), cudaMemcpyDeviceToDevice, stream));
 }
 
+void UNetEngine::set_low_res(const float* low_res_dev, cudaStream_t stream) {
+  DDNM_CHECK(lowres_ > 0, "set_low_res on a network without a low-resolution input");
+  DDNM_CHECK(low_res_dev != nullptr, "null low_res");
+  if (low_res_dev != lowres_in_)
+    CUDA_CHECK(cudaMemcpyAsync(lowres_in_, low_res_dev, (size_t)B_ * in_ch_ * lowres_ * lowres_ * 4, cudaMemcpyDeviceToDevice, stream));
+  lowres_set_ = true;
+}
+
 void UNetEngine::forward(const float* x, const float* t, float* out, cudaStream_t stream) {
   DDNM_CHECK(finalized_, "forward before finalize");
+  DDNM_CHECK(lowres_ == 0 || lowres_set_, "super-resolution network: no low_res conditioning image was given");
   const size_t xin = (size_t)B_ * in_ch_ * R_ * R_ * 4;
   if (x != x_in_) CUDA_CHECK(cudaMemcpyAsync(x_in_, x, xin, cudaMemcpyDeviceToDevice, stream));
   if (t != t_in_) CUDA_CHECK(cudaMemcpyAsync(t_in_, t, (size_t)B_ * 4, cudaMemcpyDeviceToDevice, stream));

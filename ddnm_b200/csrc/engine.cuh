@@ -52,6 +52,7 @@ struct OpenAICfg {
   int out_channels = 6, in_channels = 3, groups = 32;
   float eps = 1e-5f;
   int num_classes = 0;   // > 0: class-conditional (label_emb [num_classes, 4*model_channels], unet.py:478-479)
+  int low_res = 0;       // > 0: SuperResModel (unet.py:667-681): the stem convolves cat([x, bilinear(low_res)]), low_res [B,3,s,s]
 };
 
 class UNetEngine {
@@ -76,6 +77,9 @@ class UNetEngine {
   int* labels_in() const { return labels_in_; }
   bool class_conditional() const { return class_cond_; }
   void set_labels(const int* labels_dev, cudaStream_t stream);
+  // super-resolution networks: the conditioning image [B, in_channels, s, s] (s = low_res_size()) every following forward reads
+  int low_res_size() const { return lowres_; }
+  void set_low_res(const float* low_res_dev, cudaStream_t stream);
   float* out_buf() const { return out_; }
   void set_use_graph(bool on) { use_graph_ = on; }
   // 3 = fp32-grade products (parity mode, default); 1 = single fp16 product per MAC (fast, NOT parity-grade). Before finalize.
@@ -142,6 +146,9 @@ class UNetEngine {
   float *x_in_ = nullptr, *t_in_ = nullptr, *out_ = nullptr;
   int* labels_in_ = nullptr;
   bool class_cond_ = false;
+  float* lowres_in_ = nullptr;   // [B][in_ch_][lowres_][lowres_] when lowres_ > 0
+  int lowres_ = 0;
+  bool lowres_set_ = false;
   // scratch
   __half *splitA_hi_ = nullptr, *splitA_lo_ = nullptr, *splitB_hi_ = nullptr, *splitB_lo_ = nullptr;
   size_t split_elems_ = 0;

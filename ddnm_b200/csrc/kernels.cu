@@ -384,6 +384,188 @@ void conv3x3_small_cin(const float* x, int Cin, const float* w, const float* bia
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Super-resolution stem: input_blocks.0 of SuperResModel (unet.py:667-681) = Conv2d(2C, ch, 3, padding=1) applied to
+// cat([x, interpolate(low_res, (H, W), mode="bilinear")], dim=1).
+//   FUSED:  channels [0, C) of the halo tile come from x, channels [C, 2C) are interpolated from low_res while the tile is
+//           built.  The low-res rows and columns the tile's bilinear taps touch (at most TH + 3 rows by TW + 3 columns when
+//           low_res is no larger than the output) are staged in shared memory first, so each low-res value is read from
+//           global memory once per tile and neither the upsampled image nor the concatenation is ever written.
+//   !FUSED: x already holds all 2C channels (the composed form: interpolate + cat + this convolution).
+// The tile layout, the two-pixel inner loop and the GroupNorm sums are those of conv_small_cin_kernel.  2C * 9 weights x 4
+// output channels per lane do not fit in registers at C = 3, so the slab's weights live in shared memory as [k][128] (one
+// conflict-free float4 per lane and tap).
+// ---------------------------------------------------------------------------------------------------------------
+namespace {
+constexpr int SR_TW = 64, SR_TH = 8;
+template <int C, bool FUSED>
+struct StemSrSmem {
+  static constexpr int KT = 2 * C * 9;
+  static constexpr int LR_R = SR_TH + 4, LR_W = SR_TW + 4;
+  static constexpr size_t W_OFF = 0;
+  static constexpr size_t TILE_OFF = W_OFF + (size_t)KT * 128 * 4;
+  static constexpr size_t LR_OFF = TILE_OFF + (size_t)2 * C * (SR_TH + 2) * (SR_TW + 2) * 4;
+  static constexpr size_t RED_OFF = LR_OFF + (FUSED ? (size_t)C * LR_R * LR_W * 4 : 0);
+  static constexpr size_t BYTES = RED_OFF + (size_t)SR_TH * 128 * 2 * 4;
+};
+}  // namespace
+
+// PyTorch's bilinear source coordinate (upsample_bilinear2d, align_corners = False, output size given):
+// src = max(scale * (dst + 0.5) - 0.5, 0) with scale = in / out; taps i0 and i0 + ip, weight l1 on the second
+__device__ __forceinline__ void bilinear_src(int dst, int in, float scale, int& i0, int& ip, float& l1) {
+  float s = fmaf(scale, (float)dst + 0.5f, -0.5f);
+  s = s < 0.f ? 0.f : s;
+  i0 = (int)s;
+  ip = i0 < in - 1 ? 1 : 0;
+  l1 = s - (float)i0;
+}
+
+template <int C, bool FUSED>
+__global__ void __launch_bounds__(256) conv_stem_sr_kernel(const float* __restrict__ x, const float* __restrict__ lr, int h, int w,
+                                                           const float* __restrict__ wgt, const float* __restrict__ bias,
+                                                           float* __restrict__ out, int H, int W, int Cout, int ld,
+                                                           StatAcc* __restrict__ stats, int st_ld) {
+  pdl_prologue();
+  using S = StemSrSmem<C, FUSED>;
+  constexpr int CIN = 2 * C, KT = S::KT, TW = SR_TW, TH = SR_TH;
+  constexpr int XC = FUSED ? C : CIN;   // channels read from x as they are
+  extern __shared__ __align__(16) unsigned char smem[];
+  float(*ws)[128] = reinterpret_cast<float(*)[128]>(smem + S::W_OFF);
+  float(*tile)[TH + 2][TW + 2] = reinterpret_cast<float(*)[TH + 2][TW + 2]>(smem + S::TILE_OFF);
+  float(*lrs)[S::LR_R][S::LR_W] = reinterpret_cast<float(*)[S::LR_R][S::LR_W]>(smem + S::LR_OFF);
+  float(*red)[128][2] = reinterpret_cast<float(*)[128][2]>(smem + S::RED_OFF);
+  const int slabs = (Cout + 127) / 128;
+  const int n = blockIdx.z / slabs;
+  const int slab = blockIdx.z % slabs;
+  const int y0 = blockIdx.y * TH;
+  const int x0 = blockIdx.x * TW;
+  for (int i = threadIdx.x; i < KT * 128; i += blockDim.x) {
+    const int k = i >> 7, col = i & 127, co = slab * 128 + col;
+    ws[k][col] = co < Cout ? __ldg(&wgt[(size_t)co * KT + k]) : 0.f;   // OIHW: k = ci*9 + ky*3 + kx
+  }
+  for (int i = threadIdx.x; i < XC * (TH + 2) * (TW + 2); i += blockDim.x) {
+    const int xx = i % (TW + 2), r = (i / (TW + 2)) % (TH + 2), c = i / ((TH + 2) * (TW + 2));
+    const int gy = y0 + r - 1, gx = x0 + xx - 1;
+    tile[c][r][xx] = (gy >= 0 && gy < H && gx >= 0 && gx < W) ? __ldg(&x[(((size_t)n * XC + c) * H + gy) * W + gx]) : 0.f;
+  }
+  if (FUSED) {
+    const float sh = (float)h / (float)H, sw = (float)w / (float)W;   // area_pixel_compute_scale
+    int ry0, cx0, ip;
+    float l1;
+    bilinear_src(max(y0 - 1, 0), h, sh, ry0, ip, l1);   // first low-res row / column any tap of this tile reads
+    bilinear_src(max(x0 - 1, 0), w, sw, cx0, ip, l1);
+    for (int i = threadIdx.x; i < C * S::LR_R * S::LR_W; i += blockDim.x) {
+      const int xx = i % S::LR_W, r = (i / S::LR_W) % S::LR_R, c = i / (S::LR_R * S::LR_W);
+      const int gy = ry0 + r, gx = cx0 + xx;
+      lrs[c][r][xx] = (gy < h && gx < w) ? __ldg(&lr[(((size_t)n * C + c) * h + gy) * w + gx]) : 0.f;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < C * (TH + 2) * (TW + 2); i += blockDim.x) {
+      const int xx = i % (TW + 2), r = (i / (TW + 2)) % (TH + 2), c = i / ((TH + 2) * (TW + 2));
+      const int gy = y0 + r - 1, gx = x0 + xx - 1;
+      float v = 0.f;
+      if (gy >= 0 && gy < H && gx >= 0 && gx < W) {
+        int a0, ap, b0, bp;
+        float ly1, lx1;
+        bilinear_src(gy, h, sh, a0, ap, ly1);
+        bilinear_src(gx, w, sw, b0, bp, lx1);
+        const float ly0 = 1.f - ly1, lx0 = 1.f - lx1;
+        const float* p0 = &lrs[c][a0 - ry0][b0 - cx0];
+        const float* p1 = p0 + ap * S::LR_W;
+        v = ly0 * (lx0 * p0[0] + lx1 * p0[bp]) + ly1 * (lx0 * p1[0] + lx1 * p1[bp]);   // upsample_bilinear2d's expression
+      }
+      tile[C + c][r][xx] = v;
+    }
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int co = slab * 128 + lane * 4;
+  const bool active = co < Cout;
+  float b4[4] = {0, 0, 0, 0};
+  if (active)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) b4[j] = __ldg(&bias[co + j]);
+  __syncthreads();
+  const int y = y0 + warp;
+  float s4[4] = {0.f, 0.f, 0.f, 0.f}, q4[4] = {0.f, 0.f, 0.f, 0.f};
+  float* orow = out + (((size_t)n * H + y) * W + x0) * ld + co;
+  for (int px = 0; active && y < H && px < TW && x0 + px < W; px += 2) {
+    float acc0[4] = {b4[0], b4[1], b4[2], b4[3]};
+    float acc1[4] = {b4[0], b4[1], b4[2], b4[3]};
+    // not unrolled over channels: the weights are loop-invariant across pixels, and a fully unrolled body makes the compiler
+    // keep all 2C * 9 * 4 of them in registers (255 registers and spills at C = 3)
+#pragma unroll 1
+    for (int c = 0; c < CIN; ++c)
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+        const float2 v01 = *reinterpret_cast<const float2*>(&tile[c][warp + r][px]);
+        const float2 v23 = *reinterpret_cast<const float2*>(&tile[c][warp + r][px + 2]);
+        const float v[4] = {v01.x, v01.y, v23.x, v23.y};
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+          const float4 wv = *reinterpret_cast<const float4*>(&ws[c * 9 + r * 3 + d][lane * 4]);
+          const float wr[4] = {wv.x, wv.y, wv.z, wv.w};
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            acc0[j] = fmaf(v[d], wr[j], acc0[j]);
+            acc1[j] = fmaf(v[d + 1], wr[j], acc1[j]);
+          }
+        }
+      }
+    *reinterpret_cast<float4*>(orow + (size_t)px * ld) = make_float4(acc0[0], acc0[1], acc0[2], acc0[3]);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      s4[j] += acc0[j];
+      q4[j] = fmaf(acc0[j], acc0[j], q4[j]);
+    }
+    if (x0 + px + 1 < W) {
+      *reinterpret_cast<float4*>(orow + (size_t)(px + 1) * ld) = make_float4(acc1[0], acc1[1], acc1[2], acc1[3]);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        s4[j] += acc1[j];
+        q4[j] = fmaf(acc1[j], acc1[j], q4[j]);
+      }
+    }
+  }
+  if (stats == nullptr) return;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    red[warp][lane * 4 + j][0] = s4[j];
+    red[warp][lane * 4 + j][1] = q4[j];
+  }
+  __syncthreads();
+  const int c = threadIdx.x & 127, which = threadIdx.x >> 7;
+  if (slab * 128 + c < Cout) {
+    float t = 0.f;
+#pragma unroll
+    for (int r = 0; r < TH; ++r) t += red[r][c][which];
+    stat_add(stats + ((size_t)n * st_ld + slab * 128 + c) * 2 + which, t);
+  }
+}
+
+void conv3x3_stem_sr(const float* x, const float* low_res, int C, int h, int w, const float* w_oihw, const float* bias, const View& out,
+                     cudaStream_t st) {
+  DDNM_CHECK(C == 3, "super-resolution stem: 3 image channels");
+  DDNM_CHECK(out.C % 4 == 0, "stem Cout % 4");
+  const bool fused = low_res != nullptr;
+  if (fused) DDNM_CHECK(h >= 1 && w >= 1 && h <= out.H && w <= out.W, "super-resolution stem: low_res must be no larger than x");
+  dim3 grid(cdiv(out.W, SR_TW), cdiv(out.H, SR_TH), out.N * cdiv(out.C, 128));
+  static bool attr_f[64] = {}, attr_u[64] = {};
+  if (fused) {
+    using S = StemSrSmem<3, true>;
+    if (first_use_on_device(attr_f))
+      CUDA_CHECK(cudaFuncSetAttribute(conv_stem_sr_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::BYTES));
+    launch_pdl(conv_stem_sr_kernel<3, true>, grid, dim3(256), S::BYTES, st, 1, x, low_res, h, w, w_oihw, bias, out.p, out.H, out.W,
+               out.C, out.ld, out.st, out.st_ld);
+  } else {
+    using S = StemSrSmem<3, false>;
+    if (first_use_on_device(attr_u))
+      CUDA_CHECK(cudaFuncSetAttribute(conv_stem_sr_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)S::BYTES));
+    launch_pdl(conv_stem_sr_kernel<3, false>, grid, dim3(256), S::BYTES, st, 1, x, low_res, h, w, w_oihw, bias, out.p, out.H, out.W,
+               out.C, out.ld, out.st, out.st_ld);
+  }
+  CUDA_CHECK(cudaGetLastError());
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Network head in one kernel: h = conv_out(nonlinearity(norm_out(h)))  (models.py:338-340; unet.py:613-617 `out`), NCHW result.
 // Cout is 3 (or 6 with learned sigma): on the tensor cores the N tile has to be padded to 64 columns and the kernel is paced by
 // streaming the A operand (0.6 ms + a 0.2 ms GroupNorm pass + the NCHW copy at 256x256, B = 16).  Here the fp32 activation is read

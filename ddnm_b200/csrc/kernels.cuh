@@ -32,6 +32,11 @@ bool head_conv_supported(const View& h, int Cout);
 void head_conv(const View& h, int groups, const float* gamma, const float* beta, float eps, const float* w_oihw, const float* bias, int Cout,
                float* out_nchw, cudaStream_t s);
 void conv3x3_small_cin(const float* x_nchw, int Cin, const float* w_oihw, const float* bias, const View& out, cudaStream_t s);
+// stem of the super-resolution UNet: 3x3 pad-1 convolution of cat([x, bilinear_upsample(low_res)]) with 2C input channels.
+// low_res != nullptr: x is [N,C,H,W], low_res [N,C,h,w] (h <= H, w <= W) is interpolated inside the kernel (nothing upsampled or
+// concatenated is written); low_res == nullptr: x is the already concatenated [N,2C,H,W].  w OIHW [Cout,2C,3,3], out NHWC view.
+void conv3x3_stem_sr(const float* x_nchw, const float* low_res_nchw, int C, int h, int w, const float* w_oihw, const float* bias,
+                     const View& out, cudaStream_t s);
 // out[n][o] = act_out( sum_k act_in(in[n][k]) * W[o][k] + bias[o] );  act: 0 none, 1 swish
 void linear(const float* in, int N, int K, const float* W, const float* bias, int O, float* out, int ldo, int act_in,
             int act_out, cudaStream_t s);

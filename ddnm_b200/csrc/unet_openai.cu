@@ -13,6 +13,8 @@ namespace ddnm {
 UNetOpenAI::UNetOpenAI(const OpenAICfg& cfg, int batch)
     : UNetEngine(batch, cfg.in_channels, cfg.out_channels, cfg.image_size, cfg.groups, cfg.eps), cfg_(cfg) {
   class_cond_ = cfg.num_classes > 0;
+  DDNM_CHECK(cfg.low_res >= 0 && cfg.low_res <= cfg.image_size, "low_res size must be in [0, image_size]");
+  lowres_ = cfg.low_res;
 }
 
 // ResBlock._forward (unet.py:236-256), use_scale_shift_norm = True.

@@ -230,14 +230,94 @@ class UNetModel(_EngineModel):
             c.attn_ds[i] = v
         c.num_head_channels, c.out_channels, c.in_channels, c.groups, c.eps = self.num_head_channels, self.out_ch, self.in_channels, 32, 1e-5
         c.num_classes = self.num_classes or 0
+        c.low_res = self._low_res_size()
         h = C.c_void_p()
         _lib.check(_lib.lib().ddnm_unet_openai_create(C.byref(c), batch, C.byref(h)))
         return h
+
+    def _low_res_size(self):
+        return 0
 
     def _freq(self):
         # nn.py:113-115
         half = self.model_channels // 2
         return torch.exp(-math.log(10000) * torch.arange(start=0, end=half, dtype=torch.float32) / half)
+
+
+class SuperResModel(UNetModel):
+    """guided_diffusion.unet.SuperResModel (unet.py:667-681): a UNetModel conditioned on a low-resolution image.  As in the
+    reference, ``in_channels`` is the image's channel count and the network is built with twice as many (the checkpoint's
+    ``input_blocks.0.0.weight`` is [ch, 2 * in_channels, 3, 3]); ``model(x, t, low_res=lr)`` (or ``model(x, t, y, low_res=lr)`` when
+    class-conditional) sees ``cat([x, interpolate(lr, x.shape[2:], mode="bilinear")])``.  The interpolation and the concatenation
+    happen inside the stem kernel: neither the upsampled image nor the concatenated input is ever written to memory.
+
+    ``small_size`` is the side of ``low_res`` the engines are built for (the reference's ``sr_create_model(large_size, small_size,
+    ...)``); it defaults to a quarter of ``image_size``."""
+
+    def __init__(self, image_size, in_channels, *args, small_size=None, **kwargs):
+        super().__init__(image_size, 2 * int(in_channels), *args, **kwargs)
+        self.image_channels = int(in_channels)
+        self.small_size = int(image_size) // 4 if small_size is None else int(small_size)
+        if not 1 <= self.small_size <= self.image_size:
+            raise ValueError(f"small_size must be in [1, image_size], got {self.small_size}")
+
+    def _low_res_size(self):
+        return self.small_size
+
+    def _create(self, batch):
+        # the engine takes the image's channel count; the doubled stem input is implied by low_res > 0
+        ch, self.in_channels = self.in_channels, self.image_channels
+        try:
+            return super()._create(batch)
+        finally:
+            self.in_channels = ch
+
+    def stage_low_res(self, low_res, rows):
+        """Copy ``low_res`` ([n, C, small_size, small_size]) into the engine that runs ``rows`` rows (padded like the other inputs);
+        every forward of that engine reads it from then on, including each step of a sampling loop."""
+        if not (isinstance(low_res, torch.Tensor) and low_res.is_cuda):
+            raise _lib.DDNMError("low_res must be a CUDA tensor")
+        n = low_res.shape[0]
+        want = (self.image_channels, self.small_size, self.small_size)
+        if low_res.dim() != 4 or tuple(low_res.shape[1:]) != want:
+            raise _lib.DDNMError(f"low_res must be [B, {want[0]}, {want[1]}, {want[2]}], got {tuple(low_res.shape)}")
+        h, eb = self.engine_for(rows)
+        lr = self.pad_rows(low_res.float().contiguous(), eb)
+        _lib.check(_lib.lib().ddnm_unet_set_low_res(h, _lib.ptr(lr), _lib.cur_stream()))
+        return h, eb
+
+    def __call__(self, x, t, y=None, low_res=None):
+        return self.forward(x, t, y, low_res=low_res)
+
+    def forward(self, x, t, y=None, low_res=None):
+        if low_res is None:
+            raise _lib.DDNMError("SuperResModel needs the low_res conditioning image")
+        if low_res.shape[0] != x.shape[0]:
+            raise _lib.DDNMError(f"{low_res.shape[0]} low_res images for a batch of {x.shape[0]}")
+        assert x.dim() == 4 and x.shape[1] == self.image_channels, "x must have the image's channel count"
+        self.stage_low_res(low_res, x.shape[0])
+        return super().forward(x, t, y)
+
+
+def sr_create_model(large_size, small_size, num_channels, num_res_blocks, learn_sigma, class_cond, use_checkpoint,
+                    attention_resolutions, num_heads, num_head_channels, num_heads_upsample, use_scale_shift_norm, dropout,
+                    resblock_updown, use_fp16):
+    """guided_diffusion.script_util.sr_create_model (:335-388), same signature; the engines are built for ``small_size``."""
+    if large_size == 512:
+        channel_mult = (1, 1, 2, 2, 4, 4)
+    elif large_size == 256:
+        channel_mult = (1, 1, 2, 2, 4, 4)
+    elif large_size == 64:
+        channel_mult = (1, 2, 3, 4)
+    else:
+        raise ValueError(f"unsupported large size: {large_size}")
+    attention_ds = [large_size // int(res) for res in attention_resolutions.split(",")]
+    return SuperResModel(image_size=large_size, in_channels=3, model_channels=num_channels, out_channels=(3 if not learn_sigma else 6),
+                         num_res_blocks=num_res_blocks, attention_resolutions=tuple(attention_ds), dropout=dropout,
+                         channel_mult=channel_mult, num_classes=(1000 if class_cond else None), use_checkpoint=use_checkpoint,
+                         num_heads=num_heads, num_head_channels=num_head_channels, num_heads_upsample=num_heads_upsample,
+                         use_scale_shift_norm=use_scale_shift_norm, resblock_updown=resblock_updown, use_fp16=use_fp16,
+                         small_size=small_size)
 
 
 def create_model(image_size, num_channels, num_res_blocks, channel_mult="", learn_sigma=False, class_cond=False,

@@ -18,7 +18,7 @@ import torch
 
 from . import _lib
 from .guidance import ClassifierCondFn
-from .model import _EngineModel
+from .model import SuperResModel, _EngineModel
 from .operators import CS, Deblurring2D, GeneralA, SRConv, _Operator
 from .schedule import alpha_bar_table, time_pairs
 
@@ -75,10 +75,10 @@ def _chunked(n_pairs, x, run_range, rows=None):
         b.record_stream(side)                               # allocated on the caller's stream, written on the side stream
 
 
-def sample_device(x, model, b, eta, A_funcs, y, sigma_y, plus, config, noise=None, cls_fn=None, seed=None, row_offset=0):
+def sample_device(x, model, b, eta, A_funcs, y, sigma_y, plus, config, noise=None, cls_fn=None, seed=None, row_offset=0, low_res=None):
     """The loop with device-resident inputs and outputs (no host copies): returns (x_0, x0_pred) CUDA tensors."""
     return _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, None, config, noise, to_host=False, seed=seed,
-                row_offset=row_offset)
+                row_offset=row_offset, low_res=low_res)
 
 
 def _noise_mode(noise, seed, row_offset):
@@ -92,7 +92,15 @@ def _noise_mode(noise, seed, row_offset):
     return _lib.noise_seed(seed, row_offset)
 
 
-def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, noise=None, to_host=True, seed=None, row_offset=0):
+def _low_res_check(model, low_res, x):
+    if isinstance(model, SuperResModel) != (low_res is not None):
+        raise ValueError("low_res goes with a SuperResModel denoiser, and only with one")
+    if low_res is not None and low_res.shape[0] != x.shape[0]:
+        raise ValueError(f"{low_res.shape[0]} low_res images for a batch of {x.shape[0]}")
+
+
+def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, noise=None, to_host=True, seed=None, row_offset=0,
+         low_res=None):
     ns = _noise_mode(noise, seed, row_offset)
     if not isinstance(model, _EngineModel):
         model = getattr(model, "module", model)          # tolerate nn.DataParallel-style wrappers
@@ -102,6 +110,7 @@ def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, n
         # these operators define no Lambda / Lambda_noise: the reference fails at its first step with the base class's
         # NotImplementedError (svd_operators.py:93-97)
         raise NotImplementedError()
+    _low_res_check(model, low_res, x)
     with torch.no_grad():
         if not x.is_cuda:
             x = x.to("cuda", non_blocking=True)            # the reference moves xs[-1] to 'cuda' itself (svd_ddnm.py:45)
@@ -123,6 +132,10 @@ def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, n
         s.plus = 1 if plus else 0
         # a ragged last batch rides on an existing bigger engine, padded (classifier guidance keeps the exact size: cls_fn sees n rows)
         eng, eb = (model.engine(n), n) if cls_fn is not None else model.engine_for(n)
+        if low_res is not None:
+            # the reference passes low_res as a model kwarg on every step (model(xt, t, low_res=...)); it is the same tensor at every
+            # step, so it is staged in the engine once and each step's forward reads it there
+            model.stage_low_res(low_res.to(x.device, non_blocking=True), eb)
         out = model.pad_rows(x, eb).clone()                 # the iterate, updated in place range by range
         x0p = torch.empty_like(out)
         yv = model.pad_rows(yv, eb)
@@ -207,13 +220,17 @@ def _native_guidance(x, model, n, cond):
     return labels, grad, _lib.lib().ddnm_classifier_guidance_fn, C.cast(C.pointer(ctx), C.c_void_p)
 
 
-def ddnm_diffusion(x, model, b, eta, A_funcs, y, cls_fn=None, classes=None, config=None, noise=None, seed=None, row_offset=0):
-    return _run(x, model, b, eta, A_funcs, y, 0.0, False, cls_fn, classes, config, noise, seed=seed, row_offset=row_offset)
+def ddnm_diffusion(x, model, b, eta, A_funcs, y, cls_fn=None, classes=None, config=None, noise=None, seed=None, row_offset=0,
+                   low_res=None):
+    """``low_res``: the conditioning image of a ``SuperResModel`` denoiser ([B, 3, small_size, small_size], model space)."""
+    return _run(x, model, b, eta, A_funcs, y, 0.0, False, cls_fn, classes, config, noise, seed=seed, row_offset=row_offset,
+                low_res=low_res)
 
 
 def ddnm_plus_diffusion(x, model, b, eta, A_funcs, y, sigma_y, cls_fn=None, classes=None, config=None, noise=None, seed=None,
-                        row_offset=0):
-    return _run(x, model, b, eta, A_funcs, y, sigma_y, True, cls_fn, classes, config, noise, seed=seed, row_offset=row_offset)
+                        row_offset=0, low_res=None):
+    return _run(x, model, b, eta, A_funcs, y, sigma_y, True, cls_fn, classes, config, noise, seed=seed, row_offset=row_offset,
+                low_res=low_res)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -255,15 +272,16 @@ class SimplifiedDegradation:
         return x
 
 
-def simplified_ddnm_plus(x, model, b, eta, degradation, y, sigma_y, config=None, noise=None, seed=None, row_offset=0):
+def simplified_ddnm_plus(x, model, b, eta, degradation, y, sigma_y, config=None, noise=None, seed=None, row_offset=0, low_res=None):
     """x: x_T (B,3,H,W); y = degradation.A(x_orig); sigma_y already doubled (diffusion.py:292).  Returns
-    ``([x_0.cpu()], [x0_pred.cpu()])`` like the SVD samplers.  ``seed`` / ``row_offset``: library-drawn noise, as in
-    ``ddnm_diffusion``."""
+    ``([x_0.cpu()], [x0_pred.cpu()])`` like the SVD samplers.  ``seed`` / ``row_offset``: library-drawn noise, ``low_res``: the
+    conditioning image of a ``SuperResModel``, as in ``ddnm_diffusion``."""
     ns = _noise_mode(noise, seed, row_offset)
     if not isinstance(model, _EngineModel):
         model = getattr(model, "module", model)
     if not isinstance(model, _EngineModel) or not isinstance(degradation, SimplifiedDegradation):
         raise TypeError("simplified_ddnm_plus needs a ddnm_b200.model denoiser and a SimplifiedDegradation")
+    _low_res_check(model, low_res, x)
     with torch.no_grad():
         if not x.is_cuda:
             x = x.to("cuda", non_blocking=True)
@@ -282,6 +300,8 @@ def simplified_ddnm_plus(x, model, b, eta, degradation, y, sigma_y, config=None,
         s.num_timesteps, s.eta, s.sigma_y, s.plus = int(config.diffusion.num_diffusion_timesteps), float(eta), float(sigma_y), 1
         out, x0p = x.clone(), torch.empty_like(x)
         eng = model.engine(n)
+        if low_res is not None:
+            model.stage_low_res(low_res.to(x.device, non_blocking=True), n)
         have_x0 = C.c_int(0)
 
         def run_range(k0, k1, chunk):

@@ -51,6 +51,9 @@ typedef struct {
   float eps;
   int num_classes;            /* 0 = unconditional; > 0 = class_cond (imagenet_256_cc.yml): label_emb.weight [num_classes, 4*ch],
                                  emb = time_embed(t) + label_emb(y) (unet.py:478-479, 651-653) */
+  int low_res;                /* 0 = UNetModel; > 0 = SuperResModel (unet.py:667-681) conditioned on a [B, in_channels, low_res,
+                                 low_res] image: input_blocks.0.0.weight is [ch, 2*in_channels, 3, 3] and sees
+                                 cat([x, interpolate(low_res, (R, R), mode="bilinear")]); set it with ddnm_unet_set_low_res */
 } ddnm_openai_cfg;
 int ddnm_unet_openai_create(const ddnm_openai_cfg* cfg, int batch, void** handle);
 /* name = key of Model.state_dict() (models.py:216-299), data = fp32 host or device, reference layout (OIHW);
@@ -65,6 +68,10 @@ int ddnm_unet_finalize(void* handle);
 int ddnm_unet_forward(void* handle, const float* x, const float* t, float* out, void* stream);
 /* class-conditional networks: `model(x, t, y)` (UNetModel.forward(x, timesteps, y), unet.py:635-653); labels = device int32 [B] */
 int ddnm_unet_forward_cond(void* handle, const float* x, const float* t, const int* labels, float* out, void* stream);
+/* super-resolution networks: the conditioning image (device fp32 NCHW [B, in_channels, low_res, low_res]) that every following
+ * forward, including those of the sampling loops, reads; copied into the handle (stream-ordered).  The upsampling and the
+ * concatenation happen inside the stem kernel. */
+int ddnm_unet_set_low_res(void* handle, const float* low_res, void* stream);
 int ddnm_unet_set_graph(void* handle, int use_cuda_graph);
 int ddnm_unet_read_tap(void* handle, const char* name, float* dst_nchw, long long capacity, void* stream);
 int ddnm_unet_info(void* handle, long long* workspace_bytes, int* launches, double* flops_per_forward);
@@ -296,6 +303,11 @@ int ddnm_conv_tc(const float* x, int N, int H, int W, int Cin, const float* w, c
                  const float* side_x, int CinSide, const float* side_w, const float* residual, float* out, void* stream);
 int ddnm_conv_direct(const float* x, int N, int H, int W, int Cin, const float* w, const float* bias, int Cout, int mode, int up2,
                      float* out, void* stream);
+/* the super-resolution stem (SuperResModel's input_blocks.0): out NHWC [N,H,W,Cout] = conv3x3(cat([x, bilinear(low_res)])) + bias
+ * with x NCHW [N,C,H,W], low_res NCHW [N,C,h,w] (h <= H, w <= W, interpolated inside the kernel) and weight OIHW [Cout,2C,3,3];
+ * low_res == NULL: x is the concatenated NCHW [N,2C,H,W].  C = 3.  iters > 0: also time `iters` launches (ms_per_iter). */
+int ddnm_conv_stem_sr(const float* x, const float* low_res, int N, int C, int H, int W, int h, int w, const float* weight,
+                      const float* bias, int Cout, float* out, int iters, float* ms_per_iter, void* stream);
 /* iters > 0: all-zero operands; iters < 0: |iters| iterations on pseudo-random operands (power-realistic) */
 int ddnm_conv_tc_bench(int N, int H, int W, int Cin, int Cout, int mode, int iters, float* ms_per_iter, double* flops);
 /* diag probe: GroupNorm+SiLU+split -> 3x3 convolution over N images in chunks of `chunk` images sharing one chunk-sized plane scratch */
