@@ -21,7 +21,8 @@ class OpenAICfg(C.Structure):
     _fields_ = [("image_size", C.c_int), ("model_channels", C.c_int), ("num_res_blocks", C.c_int), ("n_levels", C.c_int),
                 ("channel_mult", C.c_int * 8), ("n_attn_ds", C.c_int), ("attn_ds", C.c_int * 4),
                 ("num_head_channels", C.c_int), ("out_channels", C.c_int), ("in_channels", C.c_int), ("groups", C.c_int),
-                ("eps", C.c_float), ("num_classes", C.c_int), ("low_res", C.c_int)]
+                ("eps", C.c_float), ("num_classes", C.c_int), ("low_res", C.c_int), ("num_heads", C.c_int),
+                ("num_heads_upsample", C.c_int), ("new_attention_order", C.c_int)]
 
 
 class ClassifierCfg(C.Structure):

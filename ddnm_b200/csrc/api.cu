@@ -48,7 +48,10 @@ int ddnm_unet_openai_create(const ddnm_openai_cfg* c, int batch, void** handle) 
   for (int i = 0; i < 4; ++i) cfg.attn_ds[i] = c->attn_ds[i];
   cfg.num_head_channels = c->num_head_channels; cfg.out_channels = c->out_channels; cfg.in_channels = c->in_channels;
   cfg.groups = c->groups; cfg.eps = c->eps; cfg.num_classes = c->num_classes; cfg.low_res = c->low_res;
+  cfg.num_heads = c->num_heads; cfg.num_heads_upsample = c->num_heads_upsample; cfg.new_attention_order = c->new_attention_order;
   DDNM_CHECK(c->num_classes >= 0, "bad num_classes");
+  DDNM_CHECK(c->new_attention_order == 0 || c->new_attention_order == 1, "new_attention_order must be 0 or 1");
+  DDNM_CHECK(c->num_head_channels > 0 || c->num_heads >= 1, "num_head_channels <= 0 needs num_heads >= 1");
   *handle = static_cast<UNetEngine*>(new UNetOpenAI(cfg, batch));
   DDNM_API_END
 }

@@ -253,8 +253,10 @@ void UNetEngine::emit_attention_core(const std::string& name, int T, int heads, 
   const long long img = (long long)T * qkv_ld;
   const double fl = 2.0 * Bn * heads * (double)T * T * ch;
   const double sbytes = (double)Bn * heads * T * T * 4;
-  if (T % 128 == 0 && ch % 64 == 0) {
-    // tensor cores: raw fp16 split of q|k|v, S = alpha Q K^T, softmax -> fp16 P, V^T planes, O = P V
+  if (T % 128 == 0 && ch % 8 == 0) {
+    // tensor cores: raw fp16 split of q|k|v, S = alpha Q K^T, softmax -> fp16 P, V^T planes, O = P V.  A head width that is not a
+    // multiple of 64 (96 in the 64 -> 256 upsampler) ends in a partial k-block of Q K^T and a partial N tile of P V (see
+    // tc_make_gemm_launch); ch % 8 keeps every head's first channel 16-byte aligned for TMA.
     __half *qh = qkvh_, *ql = qkvl_, *ph = ph_, *pl = pl_, *vh = vth_, *vl = vtl_;
     // the raw split is elementwise, so the [token][qkv_ld] buffer is viewed as rows of C = heads*ch channels (<= MAX_C)
     DDNM_CHECK(qkv_ld % C == 0, "qkv row is not a multiple of the attention width");

@@ -53,6 +53,10 @@ struct OpenAICfg {
   float eps = 1e-5f;
   int num_classes = 0;   // > 0: class-conditional (label_emb [num_classes, 4*model_channels], unet.py:478-479)
   int low_res = 0;       // > 0: SuperResModel (unet.py:667-681): the stem convolves cat([x, bilinear(low_res)]), low_res [B,3,s,s]
+  // heads per attention block when num_head_channels <= 0 (unet.py:277-283): num_heads in the input and middle blocks,
+  // num_heads_upsample (<= 0: num_heads, unet.py:452-453) in the output blocks
+  int num_heads = 1, num_heads_upsample = -1;
+  int new_attention_order = 0;   // 1: QKVAttention (q, k, v split before the heads, unet.py:361-389); 0: QKVAttentionLegacy
 };
 
 class UNetEngine {
@@ -115,7 +119,8 @@ class UNetEngine {
                  const TcWeights& w, int Cout, const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr);
   // softmax(alpha * Q K^T) V for `heads` heads of width ch over T tokens; q/k/v live in the fp32 qkv_ buffer
   // ([token][qkv_ld], head h at column h*head_stride + {q_off, k_off, v_off}); result -> attO_ [token][heads*ch].
-  // T % 128 == 0 runs both contractions on the tensor cores, otherwise (8x8 maps) on CUDA cores.
+  // T % 128 == 0 and ch % 8 == 0 run both contractions on the tensor cores (a head width that is not a multiple of 64 ends in a
+  // zero-filled partial k-block / N tile), otherwise (8x8 maps) on CUDA cores.
   void emit_attention_core(const std::string& name, int T, int heads, int ch, int qkv_ld, int head_stride, int q_off, int k_off,
                            int v_off, float alpha);
   void alloc_attention(size_t qkv_elems, size_t s_elems, size_t o_elems);
@@ -187,7 +192,9 @@ class UNetOpenAI : public UNetEngine {
   enum ResKind { RES_PLAIN = 0, RES_DOWN = 1, RES_UP = 2 };
   void build_program() override;
   void emit_resblock(const std::string& p, const View& x, const View& out, int kind);
-  void emit_attn(const std::string& p, const View& x, const View& out);
+  // heads of an attention block over C channels; upsample: the block belongs to the output blocks
+  int attn_heads(int C, bool upsample) const;
+  void emit_attn(const std::string& p, const View& x, const View& out, int heads);
   OpenAICfg cfg_;
   float* ss_all_ = nullptr;     // [B][ss_total_] scale|shift rows of every ResBlock (emb_layers outputs)
   int ss_total_ = 0;

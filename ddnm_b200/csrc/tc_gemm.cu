@@ -231,8 +231,9 @@ __device__ __forceinline__ void tc_produce_tile(const CUtensorMap* tm_a0h, const
 // Epilogue of one m64 accumulator fragment: rows r0 and r0 + 8 of the output tile, 2 adjacent columns per 8-column group.
 // out = alpha * acc + chanadd + residual (res_mode 0 / 1 / 2), or alpha * acc into split-K partial `split_off`.  The stored values
 // (0 for rows past the batch) are written back to d for the GroupNorm sums.  DUAL (dual set): the hi*lo partial sums of the same
-// columns are kept BN columns further on and added first.
-template <int BN, bool DUAL, int R>
+// columns are kept BN columns further on and added first.  NTAIL (batched GEMMs whose N is not a multiple of BN): columns at or past
+// p.Cout are not stored — in the attention output they belong to the next head.
+template <int BN, bool DUAL, bool NTAIL, int R>
 __device__ __forceinline__ void tc_epilogue_rows(const TcParams& p, float (&d)[R], bool dual, int r0, int cq, int n_idx, int x0,
                                                  int y0, int n0, int split_off) {
   const int ppi = p.bw * p.bh;
@@ -294,7 +295,7 @@ __device__ __forceinline__ void tc_epilogue_rows(const TcParams& p, float (&d)[R
       if (!valid[h]) v0 = v1 = 0.f;
       d[4 * j + 2 * h] = v0;
       d[4 * j + 2 * h + 1] = v1;
-      if (valid[h]) *reinterpret_cast<float2*>(orow[h] + c) = make_float2(v0, v1);
+      if (valid[h] && (!NTAIL || n_idx * BN + c < p.Cout)) *reinterpret_cast<float2*>(orow[h] + c) = make_float2(v0, v1);
     }
   }
 }
@@ -319,7 +320,7 @@ __device__ __forceinline__ void tc_stats_rows(const float (&d)[R], float2* part,
   }
 }
 
-template <int BN, bool PAIR, bool DUAL, bool GN, bool HALO>
+template <int BN, bool PAIR, bool DUAL, bool GN, bool HALO, bool NTAIL>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant__ CUtensorMap tm_a0l,
                const __grid_constant__ CUtensorMap tm_a1h, const __grid_constant__ CUtensorMap tm_a1l,
@@ -586,7 +587,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
     // ---- epilogue: rows r0 and r0 + 8 of this tile, 2 adjacent columns per 8-column group ----
     int n_idx, x0, y0, n0;
     decode(tile_of(u), n_idx, x0, y0, n0);
-    tc_epilogue_rows<BN, DUAL>(p, d, dual, r0, cq, n_idx, x0, y0, n0, PAIR ? 0 : u % p.split_k);
+    tc_epilogue_rows<BN, DUAL, NTAIL>(p, d, dual, r0, cq, n_idx, x0, y0, n0, PAIR ? 0 : u % p.split_k);
     if (p.stats) {
       // GroupNorm statistics of the tile.  (1) per warp: the column sums over its 16 rows (one image: >= 32 pixels per image),
       // reduced across the 8 lanes that share a column pair; (2) per image slot: the warps of that image added in a fixed order
@@ -653,7 +654,7 @@ struct PpCfg {
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory capacity");
 };
 
-template <int BN, int TERMS, bool HALO>
+template <int BN, int TERMS, bool HALO, bool NTAIL>
 __global__ void __launch_bounds__(kPpThreads, 1)
 conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant__ CUtensorMap tm_a0l,
                         const __grid_constant__ CUtensorMap tm_a1h, const __grid_constant__ CUtensorMap tm_a1l,
@@ -816,7 +817,7 @@ conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid
     int n_idx, x0, y0, n0;
     tc_decode(p, u / p.split_k, n_idx, x0, y0, n0);
 #pragma unroll
-    for (int f = 0; f < 2; ++f) tc_epilogue_rows<BN, false>(p, d[f], false, 64 * f + r0, cq, n_idx, x0, y0, n0, u % p.split_k);
+    for (int f = 0; f < 2; ++f) tc_epilogue_rows<BN, false, NTAIL>(p, d[f], false, 64 * f + r0, cq, n_idx, x0, y0, n0, u % p.split_k);
     if (p.stats) {
       // GroupNorm statistics of the tile, as in conv_tc_kernel: (1) per 16-row group (warp wq of fragment f = group 4 f + wq), the
       // column sums, (2) per image slot the groups of that image in a fixed order, into a running (value, compensation) pair that
@@ -1051,7 +1052,9 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
                              long long out_sn, long long out_sy, long long out_sx, float alpha, int num_sms) {
   TcLaunch L;
   TcParams& p = L.p;
-  DDNM_CHECK(M % 128 == 0 && N % 64 == 0 && K % BK == 0, "attention GEMM: M % 128, N % 64, K % 64");
+  // K and N need not fill whole 64-wide blocks: the operand maps end at K and N, so TMA zero-fills the rest of the last k-block and
+  // of the last N tile, and the epilogue stores no column past N (NTAIL).  The 16-byte TMA alignment of the rows needs K % 8 == 0.
+  DDNM_CHECK(M % 128 == 0 && N % 8 == 0 && K % 8 == 0, "attention GEMM: M % 128, N % 8, K % 8");
   p.H = heads; p.W = M; p.N = images;
   p.bw = 128; p.bh = 1; p.bn = 1;
   p.tiles_x = M / 128; p.tiles_y = heads; p.tiles_n = images;
@@ -1061,9 +1064,10 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
   if (N % 128 == 0 && (long long)m_tiles * (N / 128) >= num_sms / 2) L.BN = 128;
   L.dual = g_dual_mode != 0;
   L.pingpong = g_pingpong_enable != 0;
-  p.n_tiles = N / L.BN;
+  p.n_tiles = cdiv(N, L.BN);
+  L.ntail = N % L.BN != 0;
   p.mode0 = TAPS_1X1;
-  p.cb0 = K / BK; p.kb0 = K / BK; p.kb1 = 0;
+  p.cb0 = cdiv(K, BK); p.kb0 = p.cb0; p.kb1 = 0;
   p.phase_stride = 0;
   p.up_py = p.up_px = 0;
   p.b_batched = 2;
@@ -1090,19 +1094,28 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
   return L;
 }
 
-template <int BN, bool PAIR, bool DUAL, bool GN = false, bool HALO = false>
+template <int BN, bool PAIR, bool DUAL, bool GN = false, bool HALO = false, bool NTAIL = false>
 static void launch_bn(const TcLaunch& L, cudaStream_t stream) {
   using Cfg = TcCfg<BN, DUAL, HALO>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set))
-    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_kernel<BN, PAIR, DUAL, GN, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  launch_pdl(conv_tc_kernel<BN, PAIR, DUAL, GN, HALO>, dim3(L.grid), dim3(kTcThreads), (size_t)Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1,
+    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_kernel<BN, PAIR, DUAL, GN, HALO, NTAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    Cfg::SMEM_BYTES));
+  launch_pdl(conv_tc_kernel<BN, PAIR, DUAL, GN, HALO, NTAIL>, dim3(L.grid), dim3(kTcThreads), (size_t)Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1,
              HALO ? L.hh : L.a0h, HALO ? L.hl : L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.p, L.g);
   CUDA_CHECK(cudaGetLastError());
 }
 
 template <int BN>
 static void launch_forms(const TcLaunch& L, cudaStream_t stream) {
+  if (L.ntail) {   // batched GEMMs with a partial N tile: N % 64 != 0, so BN = 64
+    if constexpr (BN == 64) {
+      if (L.dual) launch_bn<BN, false, true, false, false, true>(L, stream);
+      else launch_bn<BN, false, false, false, false, true>(L, stream);
+      return;
+    }
+    throw Error("partial N tiles need BN = 64");
+  }
   if (L.halo && L.dual) launch_bn<BN, false, true, false, true>(L, stream);
   else if (L.halo) launch_bn<BN, false, false, false, true>(L, stream);
   else if (L.gn && L.dual) launch_bn<BN, false, true, true>(L, stream);
@@ -1113,19 +1126,28 @@ static void launch_forms(const TcLaunch& L, cudaStream_t stream) {
   else launch_bn<BN, false, false>(L, stream);
 }
 
-template <int BN, int TERMS, bool HALO>
+template <int BN, int TERMS, bool HALO, bool NTAIL = false>
 static void launch_pingpong(const TcLaunch& L, cudaStream_t stream) {
   using Cfg = PpCfg<BN, HALO>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set))
-    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_pingpong_kernel<BN, TERMS, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  launch_pdl(conv_tc_pingpong_kernel<BN, TERMS, HALO>, dim3(L.grid), dim3(kPpThreads), (size_t)Cfg::SMEM_BYTES, stream, 1,
+    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_pingpong_kernel<BN, TERMS, HALO, NTAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    Cfg::SMEM_BYTES));
+  launch_pdl(conv_tc_pingpong_kernel<BN, TERMS, HALO, NTAIL>, dim3(L.grid), dim3(kPpThreads), (size_t)Cfg::SMEM_BYTES, stream, 1,
              HALO ? L.hh : L.a0h, HALO ? L.hl : L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.p);
   CUDA_CHECK(cudaGetLastError());
 }
 
 template <int BN>
 static void launch_pingpong_forms(const TcLaunch& L, cudaStream_t stream) {
+  if (L.ntail) {   // as in launch_forms
+    if constexpr (BN == 64) {
+      if (L.p.terms == 1) launch_pingpong<BN, 1, false, true>(L, stream);
+      else launch_pingpong<BN, 3, false, true>(L, stream);
+      return;
+    }
+    throw Error("partial N tiles need BN = 64");
+  }
   if (L.p.terms == 1) {
     if (L.halo) launch_pingpong<BN, 1, true>(L, stream);
     else launch_pingpong<BN, 1, false>(L, stream);

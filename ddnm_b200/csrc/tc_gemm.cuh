@@ -68,6 +68,7 @@ struct TcLaunch {
   bool gn = false;             // GN form: A produced in the kernel from g
   bool halo = false;           // HALO form: one A load per (dy, channel slice) feeds the dx taps; needs split_k == 1
   bool pingpong = false;       // ping-pong kernel where the launch allows it (see tc_run); DUAL does not apply there
+  bool ntail = false;          // batched GEMM whose N is not a multiple of BN: the last N tile is partial (never a convolution)
   TcGnArgs g;
   int grid = 0;
   double flops = 0;            // algorithmic flops (2*M*N*K, counted once)
@@ -85,14 +86,15 @@ TcLaunch tc_make_up2_launch(const SplitView& src, const __half* w_hi, const __ha
                             int ca_ld, int py, int px, int num_sms);
 
 // Strided fp16 (hi, lo) operand for the batched-GEMM builder: element (k, row, head, image) at
-// base[k + row*s_row + head*s_head + image*s_img]; k extent = K (multiple of 64).
+// base[k + row*s_row + head*s_head + image*s_img]; k extent = K (multiple of 8; base and strides 16-byte aligned).
 struct GemmOperand {
   const __half* hi;
   const __half* lo;
   long long s_row, s_head, s_img;
 };
 // out[img*out_sn + head*out_sy + m*out_sx + n] = alpha * sum_k A[k, m, head, img] * B[k, n, head, img]
-// (multi-head attention: QK^T and PV).  M % 128 == 0, N % 64 == 0, K % 64 == 0.
+// (multi-head attention: QK^T and PV).  M % 128 == 0, N % 8 == 0, K % 8 == 0: a partial last k-block / N tile is zero-filled by
+// TMA, and no column past N is stored.
 TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, int N, int K, int heads, int images, float* out,
                              long long out_sn, long long out_sy, long long out_sx, float alpha, int num_sms);
 

@@ -1,5 +1,6 @@
-// UNetOpenAI: launch program for guided_diffusion/unet.py::UNetModel as configured by imagenet_256.yml
-// (use_scale_shift_norm, resblock_updown, legacy multi-head attention with 64-channel heads, learn_sigma -> 6 outputs).
+// UNetOpenAI: launch program for guided_diffusion/unet.py::UNetModel as configured by imagenet_256.yml and the rest of the
+// guided-diffusion ImageNet family (use_scale_shift_norm, resblock_updown; legacy or new attention order, heads of num_head_channels
+// channels or a fixed count per block; learn_sigma -> 6 outputs).
 // Everything is computed with fp32-grade arithmetic (the reference's fp32 mode); its optional fp16 torso
 // (unet.py:619-625) is a lower-precision variant of the same maths.
 #include <algorithm>
@@ -68,18 +69,31 @@ void UNetOpenAI::emit_resblock(const std::string& p, const View& x, const View& 
   }
 }
 
-// AttentionBlock._forward (unet.py:299-305) with QKVAttentionLegacy (:337-354): qkv channels are laid out per head as
-// [q(ch) | k(ch) | v(ch)], ch = 64; weight = softmax((q*s)^T (k*s)), s = ch^-1/4; a = weight . v
-void UNetOpenAI::emit_attn(const std::string& p, const View& x, const View& out) {
-  const int C = x.C, T = x.H * x.W, ch = cfg_.num_head_channels, heads = C / ch;
-  DDNM_CHECK(C % ch == 0, "channels not divisible by num_head_channels");
+// AttentionBlock.__init__ (unet.py:277-283, 452-453): num_head_channels-wide heads, else a fixed count per block
+int UNetOpenAI::attn_heads(int C, bool upsample) const {
+  int heads = cfg_.num_heads;
+  if (cfg_.num_head_channels > 0) heads = C / cfg_.num_head_channels;
+  else if (upsample && cfg_.num_heads_upsample > 0) heads = cfg_.num_heads_upsample;
+  DDNM_CHECK(heads >= 1 && C % heads == 0 && (cfg_.num_head_channels <= 0 || C % cfg_.num_head_channels == 0),
+             "attention channels " + std::to_string(C) + " do not split into equal heads");
+  return heads;
+}
+
+// AttentionBlock._forward (unet.py:299-305); weight = softmax((q*s)^T (k*s)), s = ch^-1/4; a = weight . v; head h of a is channels
+// [h*ch, (h+1)*ch) in both orders.  The qkv channels of head h are
+//   QKVAttentionLegacy (:337-354): [q | k | v] at h*3ch + {0, ch, 2ch}   (heads split before q, k, v)
+//   QKVAttention (:361-389):       h*ch + {0, C, 2C}                    (q, k, v split before the heads)
+void UNetOpenAI::emit_attn(const std::string& p, const View& x, const View& out, int heads) {
+  const int C = x.C, T = x.H * x.W, ch = C / heads;
   SplitView A{splitA_hi_, splitA_lo_};
   emit_gn_split(p + ".norm", x, p + ".norm", false, SPLIT_SAME, A);
   TcWeights wqkv = prep_weights(p + ".qkv.weight", 3 * C, C, 1, "", 0);
   View qkv;
   qkv.p = qkv_; qkv.N = B_; qkv.H = x.H; qkv.W = x.W; qkv.C = 3 * C; qkv.ld = 3 * C;
   emit_tc(p + ".qkv", A, TAPS_1X1, nullptr, wqkv, 3 * C, qkv, P(p + ".qkv.bias", 3 * C), 0, nullptr, 0);
-  emit_attention_core(p, T, heads, ch, 3 * C, 3 * ch, 0, ch, 2 * ch, 1.0f / std::sqrt((float)ch));  // (ch^-1/4)^2
+  const float alpha = 1.0f / std::sqrt((float)ch);   // (ch^-1/4)^2
+  if (cfg_.new_attention_order) emit_attention_core(p, T, heads, ch, 3 * C, ch, 0, C, 2 * C, alpha);
+  else emit_attention_core(p, T, heads, ch, 3 * C, 3 * ch, 0, ch, 2 * ch, alpha);
   View ov;
   ov.p = attO_; ov.N = B_; ov.H = x.H; ov.W = x.W; ov.C = C; ov.ld = C;
   emit_gn_split(p + ".proj_in", ov, "", false, SPLIT_SAME, A);
@@ -168,7 +182,7 @@ void UNetOpenAI::build_program() {
         rb_cout.push_back(l.cout);
         r = ro;
       } else if (l.kind == 4) {
-        const size_t T = (size_t)r * r, heads = l.cin / c.num_head_channels;
+        const size_t T = (size_t)r * r, heads = attn_heads(l.cin, prefix.rfind("output_blocks", 0) == 0);
         split_max = std::max(split_max, (size_t)B_ * T * l.cin);
         att_qkv = std::max(att_qkv, (size_t)B_ * T * 3 * l.cin);
         att_S = std::max(att_S, (size_t)B_ * heads * T * T);
@@ -253,7 +267,7 @@ void UNetOpenAI::build_program() {
       if (l.kind == 3) ro = cur.H * 2;
       View dst = last ? final_dst : new_view(ro, ro, l.cout);
       DDNM_CHECK(dst.H == ro && dst.C == l.cout, "layer destination shape");
-      if (l.kind == 4) emit_attn(p, cur, dst);
+      if (l.kind == 4) emit_attn(p, cur, dst, attn_heads(cur.C, prefix.rfind("output_blocks", 0) == 0));
       else emit_resblock(p, cur, dst, l.kind == 2 ? RES_DOWN : (l.kind == 3 ? RES_UP : RES_PLAIN));
       cur = dst;
     }

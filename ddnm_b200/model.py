@@ -185,17 +185,27 @@ class Model(_EngineModel):
 
 
 class UNetModel(_EngineModel):
-    """guided_diffusion.unet.UNetModel (unet.py:396-664) for the variant the shipped configs build
-    (use_scale_shift_norm, resblock_updown, legacy attention order; optional class conditioning: ``model(x, t, y)``)."""
+    """guided_diffusion.unet.UNetModel (unet.py:396-664) for the variants guided-diffusion's ImageNet models use
+    (use_scale_shift_norm, resblock_updown; either attention order; heads of ``num_head_channels`` channels, or when it is -1 a
+    fixed ``num_heads`` in the input and middle blocks and ``num_heads_upsample`` in the output blocks; optional class
+    conditioning: ``model(x, t, y)``)."""
 
     def __init__(self, image_size, in_channels, model_channels, out_channels, num_res_blocks, attention_resolutions,
                  dropout=0, channel_mult=(1, 2, 4, 8), conv_resample=True, dims=2, num_classes=None, use_checkpoint=False,
                  use_fp16=False, num_heads=1, num_head_channels=-1, num_heads_upsample=-1, use_scale_shift_norm=False,
                  resblock_updown=False, use_new_attention_order=False):
         self.num_classes = None if num_classes is None else int(num_classes)   # label_emb (unet.py:478-479), imagenet_256_cc.yml
-        if not (use_scale_shift_norm and resblock_updown) or use_new_attention_order or num_head_channels <= 0 or dims != 2:
-            raise NotImplementedError("ddnm_b200 builds the imagenet_256.yml UNetModel variant: use_scale_shift_norm, "
-                                      "resblock_updown, legacy attention order, num_head_channels > 0")
+        if not (use_scale_shift_norm and resblock_updown) or dims != 2:
+            raise NotImplementedError("ddnm_b200 builds the guided-diffusion ImageNet UNetModel variants: use_scale_shift_norm, "
+                                      "resblock_updown")
+        # AttentionBlock.__init__ (unet.py:277-283): -1 means a fixed head count; anything else is the head width
+        if not (int(num_head_channels) > 0 or (int(num_head_channels) == -1 and int(num_heads) >= 1)):
+            raise ValueError(f"num_head_channels must be -1 (use num_heads) or positive, got {num_head_channels} with "
+                             f"num_heads={num_heads}")
+        if int(num_heads_upsample) == -1:      # unet.py:452-453
+            num_heads_upsample = num_heads
+        if int(num_head_channels) == -1 and int(num_heads_upsample) < 1:
+            raise ValueError(f"num_heads_upsample must be -1 or positive, got {num_heads_upsample}")
         self.image_size = self.resolution = int(image_size)
         self.in_channels, self.model_channels, self.out_ch = int(in_channels), int(model_channels), int(out_channels)
         self.out_channels = self.out_ch
@@ -207,6 +217,8 @@ class UNetModel(_EngineModel):
             raise NotImplementedError(f"ddnm_b200 UNetModel: non-integer channel multipliers {tuple(channel_mult)} are not built")
         self.channel_mult = tuple(int(v) for v in channel_mult)
         self.num_head_channels = int(num_head_channels)
+        self.num_heads, self.num_heads_upsample = int(num_heads), int(num_heads_upsample)
+        self.use_new_attention_order = bool(use_new_attention_order)
         self.use_fp16 = bool(use_fp16)
         self.dtype = torch.float32       # the engine always computes with fp32-grade arithmetic
         self._init_common()
@@ -231,6 +243,8 @@ class UNetModel(_EngineModel):
         c.num_head_channels, c.out_channels, c.in_channels, c.groups, c.eps = self.num_head_channels, self.out_ch, self.in_channels, 32, 1e-5
         c.num_classes = self.num_classes or 0
         c.low_res = self._low_res_size()
+        c.num_heads, c.num_heads_upsample = self.num_heads, self.num_heads_upsample
+        c.new_attention_order = 1 if self.use_new_attention_order else 0
         h = C.c_void_p()
         _lib.check(_lib.lib().ddnm_unet_openai_create(C.byref(c), batch, C.byref(h)))
         return h

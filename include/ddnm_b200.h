@@ -37,8 +37,10 @@ typedef struct {
 
 int ddnm_unet_simple_create(const ddnm_simple_cfg* cfg, int batch, void** handle);
 
-/* Denoiser: guided_diffusion/unet.py::UNetModel as built by script_util.create_model (:130-185) for imagenet_256.yml:
- * use_scale_shift_norm, resblock_updown, legacy attention order, class_cond = false.  Replaces `et = model(xt, t)` for
+/* Denoiser: guided_diffusion/unet.py::UNetModel as built by script_util.create_model (:130-185) for imagenet_256.yml and the
+ * rest of the guided-diffusion ImageNet family (64 / 128 / 256 base models, the SuperResModel upsamplers): use_scale_shift_norm,
+ * resblock_updown, either attention order, heads of num_head_channels channels or a fixed num_heads / num_heads_upsample per block,
+ * optional class conditioning.  Replaces `et = model(xt, t)` for
  * model.type == "openai" (UNetModel.forward, unet.py:635-664).  Parameter names = UNetModel.state_dict() keys
  * (Conv1d qkv / proj_out weights keep their (O, I, 1) layout); "__freq" = exp(-log(1e4) * arange(mc/2) / (mc/2))
  * (nn.py:113-115).  All handle functions below (set_param ... destroy) accept either denoiser kind. */
@@ -54,6 +56,10 @@ typedef struct {
   int low_res;                /* 0 = UNetModel; > 0 = SuperResModel (unet.py:667-681) conditioned on a [B, in_channels, low_res,
                                  low_res] image: input_blocks.0.0.weight is [ch, 2*in_channels, 3, 3] and sees
                                  cat([x, interpolate(low_res, (R, R), mode="bilinear")]); set it with ddnm_unet_set_low_res */
+  int num_heads;              /* used when num_head_channels <= 0 (unet.py:277-283): heads of the input- and middle-block attention */
+  int num_heads_upsample;     /* ... and of the output-block attention; <= 0 = num_heads (unet.py:452-453) */
+  int new_attention_order;    /* 0 = QKVAttentionLegacy (heads split before q, k, v); 1 = QKVAttention (q, k, v split first,
+                                 unet.py:361-389).  All-zero new fields = the layout before they existed */
 } ddnm_openai_cfg;
 int ddnm_unet_openai_create(const ddnm_openai_cfg* cfg, int batch, void** handle);
 /* name = key of Model.state_dict() (models.py:216-299), data = fp32 host or device, reference layout (OIHW);
