@@ -134,6 +134,7 @@ _SIGS = {
     "ddnm_tc_debug_pair_mode": (C.c_int, [_I]),
     "ddnm_tc_debug_halo": (C.c_int, [_I]),
     "ddnm_tc_debug_pingpong": (C.c_int, [_I]),
+    "ddnm_tc_debug_pp_pair": (C.c_int, [_I]),
 }
 EXPORTS = ["ddnm_last_error"] + list(_SIGS)
 

@@ -535,6 +535,11 @@ int ddnm_tc_debug_pingpong(int on) {
   tc_debug_pingpong(on);
   DDNM_API_END
 }
+int ddnm_tc_debug_pp_pair(int on) {
+  DDNM_API_BEGIN
+  tc_debug_pp_pair(on);
+  DDNM_API_END
+}
 int ddnm_tc_debug_force_bn(int bn) {
   DDNM_API_BEGIN
   tc_debug_force_bn(bn);

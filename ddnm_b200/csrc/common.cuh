@@ -250,11 +250,13 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster
+// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster.  The callers only hand back a stage whose
+// wgmma reads have completed (wgmma.wait_group), so the arrive publishes no memory writes: with the default .cta scope it is a
+// plain remote arrive, where .release.cluster would put a MEMBAR.ALL.GPU in front of every k-block's release.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 // TMA load written to the same shared-memory offset in every CTA of `mask`, each completing bytes on its own barrier at `bar`
 __device__ __forceinline__ void tma_load_3d_multicast(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, uint16_t mask) {

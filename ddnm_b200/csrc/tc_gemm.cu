@@ -138,18 +138,20 @@ struct TcRing {
 // TMA loads of the k-blocks [kb_lo, kb_hi) of one output tile, issued by one thread: per k-block the B planes into the next stage
 // and the A operand — the tap-shifted window (3x3, stride-2 phase, upsample phase), the 1x1 side input, or (HALO) one halo unit
 // per (dy, channel slice) at its first dx k-block.  GN: only the B planes (the consumers write A).  PAIR: this CTA's half of the B
-// tile, multicast into both CTAs of the pair.
+// tile, multicast into both CTAs of the pair.  load_a == false (PAIR only): the B halves alone, in the k order of `tile`, for a peer
+// CTA that has one unit more than this one.
 template <class Cfg, bool PAIR, bool GN, bool HALO>
 __device__ __forceinline__ void tc_produce_tile(const CUtensorMap* tm_a0h, const CUtensorMap* tm_a0l, const CUtensorMap* tm_a1h,
                                                 const CUtensorMap* tm_a1l, const CUtensorMap* tm_bh, const CUtensorMap* tm_bl,
                                                 const TcParams& p, uint32_t smem_base, TcBars<Cfg::STAGES> bars, int tile, int kb_lo,
-                                                int kb_hi, uint32_t rank, TcRing& r) {
+                                                int kb_hi, uint32_t rank, TcRing& r, bool load_a = true) {
   const int halo_r = p.mode0 == TAPS_UP2X2 ? 2 : 3;
   const int halo_w = p.bw + halo_r - 1;
   const bool lo = p.terms != 1;
   const uint32_t planes = lo ? 2u : 1u;
   // GN / HALO: only the B planes arrive with a stage (GN: the consumers write A themselves)
-  const uint32_t stage_tx = (GN || HALO) ? planes * Cfg::B_PLANE_BYTES : (uint32_t)(lo ? Cfg::STAGE_BYTES : Cfg::STAGE_BYTES / 2);
+  const uint32_t stage_tx = (GN || HALO || !load_a) ? planes * Cfg::B_PLANE_BYTES
+                                                    : (uint32_t)(lo ? Cfg::STAGE_BYTES : Cfg::STAGE_BYTES / 2);
   int n_idx, x0, y0, n0;
   tc_decode(p, tile, n_idx, x0, y0, n0);
   const int bz = p.b_batched == 1 ? n0 : 0;
@@ -159,7 +161,7 @@ __device__ __forceinline__ void tc_produce_tile(const CUtensorMap* tm_a0h, const
       // k order (dy, slice, dx); a new A unit at dx == 0
       const int ua = kb / halo_r, dx = kb - ua * halo_r, dy = ua / p.cb0, cs = ua - dy * p.cb0;
       bkb = (dy * halo_r + dx) * p.cb0 + cs;
-      if (dx == 0) {
+      if (dx == 0 && load_a) {
         mbar_wait(bars.a_empty(r.aunit), r.aphase ^ 1u);
         const uint32_t ua_s = smem_base + r.aunit * Cfg::A_UNIT_BYTES;
         const uint32_t fa = bars.a_full(r.aunit);
@@ -181,7 +183,7 @@ __device__ __forceinline__ void tc_produce_tile(const CUtensorMap* tm_a0h, const
     const uint32_t sb = HALO ? sa : sa + 2 * A_PLANE_BYTES;
     const uint32_t fb = bars.full(r.stage);
     mbar_expect_tx(fb, stage_tx);
-    if (GN || HALO) {
+    if (GN || HALO || !load_a) {
     } else if (kb < p.kb0) {
       const int tap = kb / p.cb0;
       const int c = (kb - tap * p.cb0) * BK;
@@ -210,8 +212,8 @@ __device__ __forceinline__ void tc_produce_tile(const CUtensorMap* tm_a0h, const
       constexpr int BN = Cfg::B_PLANE_BYTES / (BK * 2);
       const uint32_t half = rank * (BN / 2) * 128u;
       const int brow = n_idx * BN + (int)rank * (BN / 2);
-      tma_load_3d_multicast(sb + half, tm_bh, fb, kb * BK, brow, 0, (uint16_t)3);
-      if (lo) tma_load_3d_multicast(sb + Cfg::B_PLANE_BYTES + half, tm_bl, fb, kb * BK, brow, 0, (uint16_t)3);
+      tma_load_3d_multicast(sb + half, tm_bh, fb, bkb * BK, brow, 0, (uint16_t)3);
+      if (lo) tma_load_3d_multicast(sb + Cfg::B_PLANE_BYTES + half, tm_bl, fb, bkb * BK, brow, 0, (uint16_t)3);
     } else if (p.b_batched == 2) {
       constexpr int BN = Cfg::B_PLANE_BYTES / (BK * 2);
       tma_load_4d(sb, tm_bh, fb, kb * BK, n_idx * BN, y0, n0);
@@ -638,8 +640,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
 // and runs the epilogue while the other warpgroup's MMAs keep the tensor cores busy.  Each output element gets the products of the
 // three-instruction form in the same order (hi*hi, hi*lo, lo*hi per 16-deep k-step), so the output is bit-identical to
 // conv_tc_kernel without DUAL.  Used for the single-CTA launches without the GN form where a CTA walks at least two tiles.
+// PAIR: clusters of two CTAs.  Each producer loads its own A and HALF of every B k-block, multicast into both CTAs, so a weight row
+// crosses L2 -> SM once per two tiles; a B stage's empty barrier counts the 4 warps of consumer c in this CTA and the 4 of consumer c
+// in the peer.  The tile -> worker deal is the unpaired one; the CTAs of cluster k act as workers w and w + T (T = n_tiles, see
+// pp_worker), whose tiles at every step have the same N tile because the grid is a multiple of 2T.  Every warpgroup thus sees the
+// same tiles in the same order as unpaired, and the output, GroupNorm sums included, is bit-identical to the unpaired launch.  When
+// the deal gives the peer one unit more, this CTA walks that step as a ghost: its producer thread multicasts its B halves and
+// releases each stage for this CTA's consumers, without MMAs.
 // -------------------------------------------------------------------------------------------------------------------
 static constexpr int kPpThreads = 384;
+
+// PAIR: the unpaired worker whose units CTA `cta` walks.  Cluster k = cta / 2 pairs workers w and w + T (T = n_tiles) of the block
+// of 2T workers it falls in; T = 1 keeps worker = cta.
+__device__ __forceinline__ int pp_worker(int cta, int T) {
+  const int k = cta >> 1;
+  return (k / T) * 2 * T + k % T + (cta & 1) * T;
+}
 
 template <int BN, bool HALO>
 struct PpCfg {
@@ -654,12 +670,13 @@ struct PpCfg {
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory capacity");
 };
 
-template <int BN, int TERMS, bool HALO, bool NTAIL>
+template <int BN, int TERMS, bool HALO, bool NTAIL, bool PAIR>
 __global__ void __launch_bounds__(kPpThreads, 1)
 conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant__ CUtensorMap tm_a0l,
                         const __grid_constant__ CUtensorMap tm_a1h, const __grid_constant__ CUtensorMap tm_a1l,
                         const __grid_constant__ CUtensorMap tm_bh, const __grid_constant__ CUtensorMap tm_bl, const TcParams p) {
   static_assert(TERMS == 1 || TERMS == 3, "1 or 3 fp16 products per MAC");
+  static_assert(!PAIR || !NTAIL, "CTA pairs share one weight matrix (no batched GEMMs)");
   using Cfg = PpCfg<BN, HALO>;
   using Ring = typename Cfg::Ring;
   constexpr int STAGES = Ring::STAGES;
@@ -672,13 +689,20 @@ conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid
   const int lane = threadIdx.x & 31;
   const int KB = p.kb0 + p.kb1;
   const int n_units = p.tiles_x * p.tiles_y * p.tiles_n * p.n_tiles * p.split_k;
-  const int n_workers = (int)gridDim.x, worker = (int)blockIdx.x;
+  const int n_workers = (int)gridDim.x, worker = PAIR ? pp_worker((int)blockIdx.x, p.n_tiles) : (int)blockIdx.x;
   // the tile -> CTA deal of conv_tc_kernel
   const int unit_begin = p.deal ? (int)((long long)worker * n_units / n_workers) : worker;
   const int unit_end = p.deal ? (int)((long long)(worker + 1) * n_units / n_workers) : n_units;
   const int unit_step = p.deal ? 1 : n_workers;
   auto k_lo = [&](int u) { return (int)((long long)(u % p.split_k) * KB / p.split_k); };
   auto k_hi = [&](int u) { return (int)((long long)(u % p.split_k + 1) * KB / p.split_k); };
+  // PAIR: units of a worker; the cluster walks max(own, peer's) steps (split_k == 1: every unit is KB k-blocks).  Only the producer
+  // warpgroup uses these: at BN = 128 the consumers' main loop has no registers to spare.
+  auto units_of = [&](int w) {
+    return p.deal ? (int)((long long)(w + 1) * n_units / n_workers) - (int)((long long)w * n_units / n_workers)
+                  : (n_units - w + n_workers - 1) / n_workers;
+  };
+  const int peer = worker + ((blockIdx.x & 1) ? -p.n_tiles : p.n_tiles);   // PAIR: the worker of the other CTA of the cluster
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_a0h);
@@ -691,7 +715,7 @@ conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid
     }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(bars.full(s), 1);    // the producer's expect_tx arrive
-      mbar_init(bars.empty(s), 4);   // one arrive per warp of the consuming warpgroup
+      mbar_init(bars.empty(s), PAIR ? 8 : 4);   // one arrive per warp of the consuming warpgroup (of both CTAs of a pair)
     }
     if (HALO) {
       for (int u = 0; u < HALO_UNITS; ++u) {
@@ -703,7 +727,8 @@ conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid
     mbar_init(bars.turn(1), 4);
     mbar_fence_init();
   }
-  __syncthreads();
+  if (PAIR) cluster_sync_all();   // the peer's barriers exist before any multicast or remote arrive can reach them
+  else __syncthreads();
 
   if (warp < 4) {
     // ------------------------------------------------ TMA producer ------------------------------------------------
@@ -711,8 +736,40 @@ conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid
     if (threadIdx.x == 0) {
       TcRing ring;
       for (int u = unit_begin; u < unit_end; u += unit_step)
-        tc_produce_tile<Ring, false, false, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars,
-                                                  u / p.split_k, k_lo(u), k_hi(u), 0u, ring);
+        tc_produce_tile<Ring, PAIR, false, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars,
+                                                 u / p.split_k, k_lo(u), k_hi(u), PAIR ? cluster_ctarank() : 0u, ring);
+      if constexpr (PAIR) {
+        const int peer_begin = p.deal ? (int)((long long)peer * n_units / n_workers) : peer;
+        // ghost steps (the peer has a unit more): this thread fills each stage with its B halves (in the peer tile's k order) and
+        // releases it for this CTA's consumers, one ring behind.  It issued that fill itself, after the stage's previous fill had been
+        // consumed, so the full barrier is at most one phase behind the wait.
+        const uint32_t g0 = (uint32_t)(units_of(worker) * KB);
+        uint32_t q = g0;
+        auto ghost_release = [&](uint32_t g) {
+          mbar_wait(bars.full(g % STAGES), (g / STAGES) & 1u);
+          for (int w = 0; w < 4; ++w) {   // the arrivals of a consumer's 4 warps, here and in the peer
+            mbar_arrive(bars.empty(g % STAGES));
+            mbar_arrive_cluster(bars.empty(g % STAGES), cluster_ctarank() ^ 1u);
+          }
+        };
+        for (int j = units_of(worker); j < units_of(peer); ++j) {
+          for (int kb = 0; kb < KB; ++kb, ++q) {
+            if (q >= g0 + STAGES) ghost_release(q - STAGES);
+            tc_produce_tile<Ring, true, false, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars,
+                                                     peer_begin + j * unit_step, kb, kb + 1, cluster_ctarank(), ring, false);
+          }
+        }
+        for (uint32_t g = q >= g0 + STAGES ? q - STAGES : g0; g < q; ++g) ghost_release(g);
+        // teardown: wait until the consumers of both CTAs have released the last fill of every stage.  After that no remote arrive
+        // can reach this CTA, and every multicast into it has been waited for by its own consumers, so it may exit.
+        for (int s = 0; s < STAGES; ++s) {
+          mbar_wait(bars.empty(ring.stage), ring.phase ^ 1u);
+          if (++ring.stage == STAGES) {
+            ring.stage = 0;
+            ring.phase ^= 1u;
+          }
+        }
+      }
     }
     return;
   }
@@ -740,7 +797,10 @@ conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid
     for (int i = tid; i < 2 * BN; i += 128) run[i] = make_float2(0.f, 0.f);
   }
   auto release = [&](int s) {
-    if (lane == 0) mbar_arrive(bars.empty(s));
+    if (lane == 0) {
+      mbar_arrive(bars.empty(s));
+      if (PAIR) mbar_arrive_cluster(bars.empty(s), cluster_ctarank() ^ 1u);
+    }
   };
   auto release_a = [&](uint32_t a) {
     if (lane == 0) mbar_arrive(bars.a_empty(a % HALO_UNITS));
@@ -926,6 +986,9 @@ void tc_debug_halo(int on) { g_halo_enable = on; }
 // them on conv_tc_kernel
 static int g_pingpong_enable = [] { const char* v = std::getenv("DDNM_PINGPONG"); return v && *v ? std::atoi(v) : 1; }();
 void tc_debug_pingpong(int on) { g_pingpong_enable = on; }
+// ping-pong launches with one N tile on CTA pairs that multicast the weights (see conv_tc_pingpong_kernel and tc_make_launch)
+static int g_pp_pair_enable = [] { const char* v = std::getenv("DDNM_PP_PAIR"); return v && *v ? std::atoi(v) : 1; }();
+void tc_debug_pp_pair(int on) { g_pp_pair_enable = on; }
 static int g_deal = -1;
 void tc_debug_deal(int mode) {
   DDNM_CHECK(mode >= -1 && mode <= 1, "deal mode must be -1 (default rule), 0 (round-robin) or 1 (contiguous ranges)");
@@ -1020,6 +1083,15 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
   const uint32_t bbox[3] = {(uint32_t)BK, (uint32_t)(L.pair ? L.BN / 2 : L.BN), 1u};   // PAIR: each CTA loads half of the B tile
   L.bh = make_map_f16(w_hi, 3, bd, bbox);
   L.bl = make_map_f16(w_lo, 3, bd, bbox);
+  // ping-pong CTA pairs (one weight matrix; tc_run takes them when the launch runs on the ping-pong kernel unsplit).  Not for the
+  // upsample phases: celeba B = 16 on an H100 SXM (700 W) ran the 128 -> 256 phases 8 % slower paired, the 256^2 / 128^2 3x3
+  // launches 3-11 % faster.
+  L.pp_pair = g_pp_pair_enable != 0 && !L.pair && w_batches == 1 && mode0 != TAPS_UP2X2;
+  if (L.pp_pair) {
+    const uint32_t hbox[3] = {(uint32_t)BK, (uint32_t)(L.BN / 2), 1u};
+    L.bh2 = make_map_f16(w_hi, 3, bd, hbox);
+    L.bl2 = make_map_f16(w_lo, 3, bd, hbox);
+  }
   const int total = p.tiles_x * p.tiles_y * p.tiles_n * p.n_tiles;
   L.grid = L.pair ? 2 * std::min(total / 2, num_sms / 2) : std::min(total, num_sms);
   // contiguous tile ranges per CTA where the GroupNorm sums of the output would otherwise be flushed at every tile: one N tile
@@ -1126,16 +1198,55 @@ static void launch_forms(const TcLaunch& L, cudaStream_t stream) {
   else launch_bn<BN, false, false>(L, stream);
 }
 
-template <int BN, int TERMS, bool HALO, bool NTAIL = false>
+template <int BN, int TERMS, bool HALO, bool NTAIL = false, bool PAIR = false>
 static void launch_pingpong(const TcLaunch& L, cudaStream_t stream) {
   using Cfg = PpCfg<BN, HALO>;
+  const auto kernel = conv_tc_pingpong_kernel<BN, TERMS, HALO, NTAIL, PAIR>;
   static bool attr_set[64] = {};
-  if (first_use_on_device(attr_set))
-    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_pingpong_kernel<BN, TERMS, HALO, NTAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    Cfg::SMEM_BYTES));
-  launch_pdl(conv_tc_pingpong_kernel<BN, TERMS, HALO, NTAIL>, dim3(L.grid), dim3(kPpThreads), (size_t)Cfg::SMEM_BYTES, stream, 1,
-             HALO ? L.hh : L.a0h, HALO ? L.hl : L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.p);
+  static int max_clusters[64] = {};
+  if (first_use_on_device(attr_set)) {
+    CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    if (PAIR) {
+      // a GPC with an odd number of free SMs holds fewer clusters of two than half its SMs
+      cudaLaunchConfig_t cfg = {};
+      cudaLaunchAttribute at;
+      at.id = cudaLaunchAttributeClusterDimension;
+      at.val.clusterDim.x = 2;
+      at.val.clusterDim.y = 1;
+      at.val.clusterDim.z = 1;
+      cfg.gridDim = dim3(2);
+      cfg.blockDim = dim3(kPpThreads);
+      cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
+      cfg.attrs = &at;
+      cfg.numAttrs = 1;
+      int dev = 0;
+      CUDA_CHECK(cudaGetDevice(&dev));
+      CUDA_CHECK(cudaOccupancyMaxActiveClusters(&max_clusters[dev & 63], kernel, &cfg));
+    }
+  }
+  if (PAIR) {
+    int dev = 0;
+    CUDA_CHECK(cudaGetDevice(&dev));
+    // the pairs keep the single-CTA grid: where its clusters cannot all be resident at once, the launch stays on single CTAs
+    if (L.grid / 2 > max_clusters[dev & 63]) {
+      launch_pingpong<BN, TERMS, HALO, NTAIL, false>(L, stream);
+      return;
+    }
+  }
+  launch_pdl(kernel, dim3(L.grid), dim3(kPpThreads), (size_t)Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1, HALO ? L.hh : L.a0h,
+             HALO ? L.hl : L.a0l, L.a1h, L.a1l, PAIR ? L.bh2 : L.bh, PAIR ? L.bl2 : L.bl, L.p);
   CUDA_CHECK(cudaGetLastError());
+}
+
+template <int BN, bool PAIR>
+static void launch_pingpong_terms(const TcLaunch& L, cudaStream_t stream) {
+  if (L.p.terms == 1) {
+    if (L.halo) launch_pingpong<BN, 1, true, false, PAIR>(L, stream);
+    else launch_pingpong<BN, 1, false, false, PAIR>(L, stream);
+  } else {
+    if (L.halo) launch_pingpong<BN, 3, true, false, PAIR>(L, stream);
+    else launch_pingpong<BN, 3, false, false, PAIR>(L, stream);
+  }
 }
 
 template <int BN>
@@ -1148,13 +1259,11 @@ static void launch_pingpong_forms(const TcLaunch& L, cudaStream_t stream) {
     }
     throw Error("partial N tiles need BN = 64");
   }
-  if (L.p.terms == 1) {
-    if (L.halo) launch_pingpong<BN, 1, true>(L, stream);
-    else launch_pingpong<BN, 1, false>(L, stream);
-  } else {
-    if (L.halo) launch_pingpong<BN, 3, true>(L, stream);
-    else launch_pingpong<BN, 3, false>(L, stream);
-  }
+  // CTA pairs: unsplit, and a grid of whole blocks of 2 * n_tiles workers, so the two workers of a cluster (pp_worker) always have
+  // the same N tile; with several N tiles the deal is round-robin (tc_make_launch)
+  if (L.pp_pair && L.p.split_k == 1 && L.grid % (2 * L.p.n_tiles) == 0 && (L.p.n_tiles == 1 || L.p.deal == 0))
+    launch_pingpong_terms<BN, true>(L, stream);
+  else launch_pingpong_terms<BN, false>(L, stream);
 }
 
 // ---- GN form: fused GroupNorm + SiLU + split + 3x3 convolution ----

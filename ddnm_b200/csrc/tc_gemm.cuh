@@ -68,6 +68,8 @@ struct TcLaunch {
   bool gn = false;             // GN form: A produced in the kernel from g
   bool halo = false;           // HALO form: one A load per (dy, channel slice) feeds the dx taps; needs split_k == 1
   bool pingpong = false;       // ping-pong kernel where the launch allows it (see tc_run); DUAL does not apply there
+  bool pp_pair = false;        // the ping-pong launch may run on CTA pairs (see tc_make_launch); bh2 / bl2 have the BN/2-row box
+  CUtensorMap bh2, bl2;
   bool ntail = false;          // batched GEMM whose N is not a multiple of BN: the last N tile is partial (never a convolution)
   TcGnArgs g;
   int grid = 0;
@@ -123,6 +125,7 @@ void tc_debug_dual_mode(int mode);   // 1 (default): DUAL form for single-CTA la
 void tc_debug_pair_dual(int on);     // 1 (default): CTA pairs use the DUAL form too, 0: the plain pair form
 void tc_debug_halo(int on);          // 1 (default, env DDNM_HALO): HALO form wherever legal, 0: never
 void tc_debug_pingpong(int on);      // 1 (default, env DDNM_PINGPONG): ping-pong kernel wherever it applies, 0: never
+void tc_debug_pp_pair(int on);       // 1 (default, env DDNM_PP_PAIR): ping-pong launches on CTA pairs where legal, 0: single CTAs
 // number of fp16 product terms used by launches built from now on (3 = parity mode, 1 = fast mode)
 void tc_set_terms(int terms);
 int tc_get_terms();

@@ -349,6 +349,9 @@ int ddnm_tc_debug_halo(int on);
  * kernel (two consumer warpgroups that each own a whole tile and take turns on the tensor cores) where a CTA gets at least two tiles;
  * 0: never */
 int ddnm_tc_debug_pingpong(int on);
+/* 1 (default, also env DDNM_PP_PAIR): ping-pong launches (not the upsample phases), built afterwards, run on clusters of two CTAs that each
+ * load half of every weight k-block and multicast it to both (bit-identical output); 0: single CTAs */
+int ddnm_tc_debug_pp_pair(int on);
 
 #ifdef __cplusplus
 }

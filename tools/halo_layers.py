@@ -1,15 +1,16 @@
 """Where a form of the wgmma convolution moves time, layer by layer, on the celeba `Model` at B = 16 (the bench workload).
---switch halo (default): the HALO form; --switch pingpong: the ping-pong kernel.
+--switch halo (default): the HALO form; --switch pingpong: the ping-pong kernel; --switch pppair: CTA pairs in the ping-pong kernel
+(not the upsample phases).
 
 1. Every celeba layer shape the HALO form applies to (3x3 stride 1 and upsample phases on maps >= 64 px wide), timed with
    `ddnm_conv_tc_bench` on pseudo-random operands, the form off and on alternately: ms, algorithmic TFLOP/s and the L2 -> shared
-   memory fill bytes per launch computed from the shape (HALO).  With --switch pingpong the epilogue features are the network's
-   (GroupNorm sums, residual, channel add).
+   memory fill bytes per launch computed from the shape (HALO; pppair: the weights once per pair of tiles).  With --switch pingpong
+   and pppair the epilogue features are the network's (GroupNorm sums, residual, channel add).
 2. One eager forward per arm (`Model.profile`, CUDA events around every launch), twice per arm in alternation: per tensor-core launch
    ms both ways, and the totals.
 
 The GPU's name, power limit and SM clocks are printed with the numbers (read-only nvidia-smi queries).
-Usage: python tools/halo_layers.py [--switch halo|pingpong] [--iters 20] [--json OUT]"""
+Usage: python tools/halo_layers.py [--switch halo|pingpong|pppair] [--iters 20] [--json OUT]"""
 import argparse
 import ctypes as C
 import json
@@ -44,7 +45,7 @@ SHAPES = [
     ("up2 64->128 256ch (phase)", 64, 256, 256, True),
 ]
 FEAT_STATS, FEAT_RES, FEAT_CHANADD, FEAT_UP2 = 16, 32, 64, 128   # ddnm_conv_tc_bench mode bits (see api.cu)
-SWITCHES = {"halo": "ddnm_tc_debug_halo", "pingpong": "ddnm_tc_debug_pingpong"}
+SWITCHES = {"halo": "ddnm_tc_debug_halo", "pingpong": "ddnm_tc_debug_pingpong", "pppair": "ddnm_tc_debug_pp_pair"}
 
 
 def gpu_info():
@@ -53,16 +54,16 @@ def gpu_info():
     return r.stdout.strip() or r.stderr.strip()
 
 
-def fill_bytes(H, W, Cin, Cout, up2, halo, bn=128):
-    """L2 -> shared-memory bytes of one launch (hi + lo planes): per tile, the weights of every k-block plus the A operand, one
-    128-row box per k-block or one halo unit per (dy, channel slice)."""
+def fill_bytes(H, W, Cin, Cout, up2, halo, bn=128, pair=False):
+    """L2 -> shared-memory bytes of one launch (hi + lo planes): per tile, the weights of every k-block (pair: half of them, the
+    other half arrives by multicast) plus the A operand, one 128-row box per k-block or one halo unit per (dy, channel slice)."""
     bw = min(W, 128)
     bh = 128 // bw
     tiles = N * H * W // 128 * (Cout // bn)
     cb = Cin // BK
     r = 2 if up2 else 3
     kb = r * r * cb
-    b = kb * 2 * bn * BK * 2
+    b = kb * 2 * bn * BK * 2 // (2 if pair else 1)
     a = r * cb * 2 * (bw + r - 1) * bh * 128 if halo else kb * 2 * 128 * BK * 2
     return tiles * (a + b)
 
@@ -71,9 +72,11 @@ def bench_shapes(L, switch, iters):
     ms, fl = C.c_float(), C.c_double()
     rows = []
     for label, H, Cin, Cout, up2 in SHAPES:
+        if switch == "ddnm_tc_debug_pp_pair" and up2:   # the upsample phases stay on single CTAs
+            continue
         # 3x3 stride 1 (mode 0) + the epilogue features the network uses (the op-level upsample phase takes no residual)
         mode = FEAT_STATS | (FEAT_UP2 if up2 else 0)
-        if switch == "ddnm_tc_debug_pingpong":
+        if switch in ("ddnm_tc_debug_pingpong", "ddnm_tc_debug_pp_pair"):
             mode |= FEAT_CHANADD | (0 if up2 else FEAT_RES)
         t = {0: [], 1: []}
         for rep in range(2):
@@ -83,8 +86,12 @@ def bench_shapes(L, switch, iters):
                 t[halo].append(ms.value)
         _lib.check(getattr(L, switch)(1))
         m0, m1 = min(t[0]), min(t[1])
+        if switch == "ddnm_tc_debug_pp_pair":   # the HALO form either way, the weights once or twice per pair of tiles
+            f0, f1 = fill_bytes(H, H, Cin, Cout, up2, True), fill_bytes(H, H, Cin, Cout, up2, True, pair=True)
+        else:
+            f0, f1 = fill_bytes(H, H, Cin, Cout, up2, False), fill_bytes(H, H, Cin, Cout, up2, True)
         rows.append(dict(layer=label, ms_off=m0, ms_on=m1, tflops_off=fl.value / m0 / 1e9, tflops_on=fl.value / m1 / 1e9,
-                         fill_mb_off=fill_bytes(H, H, Cin, Cout, up2, False) / 1e6, fill_mb_on=fill_bytes(H, H, Cin, Cout, up2, True) / 1e6))
+                         fill_mb_off=f0 / 1e6, fill_mb_on=f1 / 1e6))
         r = rows[-1]
         print(f"{label:28s} {r['ms_off']:8.3f} {r['ms_on']:8.3f} {100 * (r['ms_on'] / r['ms_off'] - 1):+6.1f}%  "
               f"{r['tflops_off']:6.1f} {r['tflops_on']:6.1f}  {r['fill_mb_off']:9.1f} {r['fill_mb_on']:9.1f}", flush=True)
