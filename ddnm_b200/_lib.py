@@ -135,6 +135,8 @@ _SIGS = {
     "ddnm_tc_debug_halo": (C.c_int, [_I]),
     "ddnm_tc_debug_pingpong": (C.c_int, [_I]),
     "ddnm_tc_debug_pp_pair": (C.c_int, [_I]),
+    "ddnm_unet_set_batch_invariant": (C.c_int, [_P, _I]),
+    "ddnm_tc_debug_sm_count": (C.c_int, [_I]),
 }
 EXPORTS = ["ddnm_last_error"] + list(_SIGS)
 

@@ -141,6 +141,11 @@ int ddnm_unet_set_precision(void* h, int fp16_terms) {
   static_cast<UNetEngine*>(h)->set_terms(fp16_terms);
   DDNM_API_END
 }
+int ddnm_unet_set_batch_invariant(void* h, int on) {
+  DDNM_API_BEGIN
+  static_cast<UNetEngine*>(h)->set_batch_invariant(on != 0);
+  DDNM_API_END
+}
 int ddnm_unet_set_graph(void* h, int on) {
   DDNM_API_BEGIN
   static_cast<UNetEngine*>(h)->set_use_graph(on != 0);
@@ -543,6 +548,11 @@ int ddnm_tc_debug_pp_pair(int on) {
 int ddnm_tc_debug_force_bn(int bn) {
   DDNM_API_BEGIN
   tc_debug_force_bn(bn);
+  DDNM_API_END
+}
+int ddnm_tc_debug_sm_count(int n) {
+  DDNM_API_BEGIN
+  engine_debug_sm_count(n);
   DDNM_API_END
 }
 }  // extern "C"

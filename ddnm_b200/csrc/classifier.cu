@@ -457,6 +457,9 @@ UNetEngine::TcWeights UNetEncoder::prep_weights_t(const std::string& name, int C
   return r;
 }
 
+// GroupNorm backward chunks per image in batch-invariant mode (256^2: 1024 pixels each; 8 images fill 4 CTAs per SM as the default does)
+static constexpr int kGnbInvariantChunks = 64;
+
 void UNetEncoder::emit_gn_backward(const std::string& name, const float* g, const View& x, const std::string& norm, const float* ss, int ss_ld,
                                    bool silu, bool pool, const float* add, bool add_pool, float* dx32, const SplitView& dst) {
   DDNM_CHECK(x.st != nullptr && x.C % groups_ == 0 && x.C <= 512, "GroupNorm backward: input without statistics / too wide");
@@ -467,7 +470,9 @@ void UNetEncoder::emit_gn_backward(const std::string& name, const float* g, cons
   A.beta = P(norm + ".bias", x.C);
   A.ss = ss; A.ss_ld = ss_ld; A.silu = silu; A.pool = pool;
   const int HW = x.H * x.W;
-  int chunks = std::max(1, std::min(HW, cdiv(4 * num_sms_, B_)));
+  // pixel chunks per image: about 4 CTAs per SM over the batch; in batch-invariant mode a fixed count, since the chunks' fp64
+  // partial sums (and so the gradient's last bits) follow the partition
+  int chunks = std::max(1, std::min(HW, invariant_ ? kGnbInvariantChunks : cdiv(4 * num_sms_, B_)));
   A.ppc = cdiv(HW, chunks);
   A.chunks = chunks = cdiv(HW, A.ppc);
   DDNM_CHECK((size_t)B_ * (chunks + 1) * x.C * 2 <= gnb_part_elems_, "GroupNorm backward partial buffer too small");
@@ -757,7 +762,7 @@ void UNetEncoder::build_program() {
   gqkv_ = (float*)arena_.alloc(act_max * 4);
   sP_ = (float*)arena_.alloc(att_S * 4);
   sdP_ = (float*)arena_.alloc(att_S * 4);
-  gnb_part_elems_ = (size_t)(4 * num_sms_ + 2 * B_) * 512 * 2;
+  gnb_part_elems_ = (size_t)(invariant_ ? B_ * (kGnbInvariantChunks + 1) : 4 * num_sms_ + 2 * B_) * 512 * 2;
   gnb_part_ = (float*)arena_.alloc(gnb_part_elems_ * sizeof(double));
 
   // ---- timestep embedding and every emb_layers Linear as one matrix (as UNetOpenAI) ----

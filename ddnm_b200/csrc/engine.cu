@@ -27,6 +27,12 @@ void* Arena::alloc(size_t bytes) {
   return p;
 }
 
+static int g_sm_count = 0;
+void engine_debug_sm_count(int n) {
+  DDNM_CHECK(n >= 0, "SM count must be 0 (the device's) or positive");
+  g_sm_count = n;
+}
+
 UNetEngine::UNetEngine(int batch, int in_channels, int out_ch, int resolution, int groups, float eps)
     : B_(batch), in_ch_(in_channels), out_ch_(out_ch), R_(resolution), groups_(groups), eps_(eps) {
   DDNM_CHECK(batch >= 1, "batch must be positive");
@@ -35,7 +41,7 @@ UNetEngine::UNetEngine(int batch, int in_channels, int out_ch, int resolution, i
   cudaDeviceProp prop;
   CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
   DDNM_CHECK(prop.major == 9 && prop.minor == 0, "ddnm_b200 kernels are built for sm_90a (H100) only");
-  num_sms_ = prop.multiProcessorCount;
+  num_sms_ = g_sm_count > 0 ? std::min(g_sm_count, prop.multiProcessorCount) : prop.multiProcessorCount;
 }
 
 UNetEngine::~UNetEngine() {
@@ -155,20 +161,26 @@ void UNetEngine::emit_gn_split(const std::string& name, const View& x, const std
 
 void UNetEngine::emit_tc(const std::string& name, const SplitView& a, int mode, const SplitView* side, const TcWeights& w,
                          int Cout, const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int res_mode) {
-  TcLaunch L = tc_make_launch(a, mode, side, w.hi, w.lo, 1, Cout, out, chanadd, ca_ld, residual, ldr, 1.0f, num_sms_, res_mode);
+  TcLaunch L = tc_make_launch(a, mode, side, w.hi, w.lo, 1, Cout, out, chanadd, ca_ld, residual, ldr, 1.0f, num_sms_, res_mode, invariant_);
   const double bytes = (double)a.N * a.H * a.W * a.C * 4 + (side ? (double)side->N * side->H * side->W * side->C * 4 : 0) +
                        (double)Cout * w.ktot * 4 + (double)out.pixels() * Cout * 4 * (residual ? 2 : 1);
   // split-K: few tiles walking a long K one k-block after the other (the 8x8 level: 32-64 CTAs, 72-144 k-blocks) are latency-bound;
   // 2 or 4 CTAs per tile, each over its own k-block range into its own partial buffer, then one small deterministic reduce
   const int tiles = L.p.tiles_x * L.p.tiles_y * L.p.tiles_n * L.p.n_tiles, kblocks = L.p.kb0 + L.p.kb1;
   static const bool split_on = std::getenv("DDNM_SPLITK") == nullptr || std::atoi(std::getenv("DDNM_SPLITK")) != 0;
-  if (split_on && !L.pair && res_mode == 0 && 2 * tiles <= num_sms_ && kblocks >= 32) {
-    const int S = 4 * tiles <= num_sms_ ? 4 : 2;
+  int S = 1;
+  if (split_on && !L.pair && res_mode == 0 && kblocks >= 32) {
+    // batch-invariant mode: S is part of an element's arithmetic (the k-block ranges and their fixed-order sum), so it follows the
+    // per-image shape alone — 2 on the maps of at most 64 pixels, the 8x8 level where B = 16 splits by the tile count as well
+    if (invariant_) S = out.H * out.W <= 64 ? 2 : 1;
+    else if (2 * tiles <= num_sms_) S = 4 * tiles <= num_sms_ ? 4 : 2;
+  }
+  if (S > 1) {
     const long long stride = out.pixels() * Cout;
     float* part = (float*)arena_.alloc((size_t)S * stride * sizeof(float));
     View pv;
     pv.p = part; pv.N = out.N; pv.H = out.H; pv.W = out.W; pv.C = Cout; pv.ld = Cout;
-    TcLaunch Ls = tc_make_launch(a, mode, side, w.hi, w.lo, 1, Cout, pv, nullptr, 0, nullptr, 0, 1.0f, num_sms_, 0);
+    TcLaunch Ls = tc_make_launch(a, mode, side, w.hi, w.lo, 1, Cout, pv, nullptr, 0, nullptr, 0, 1.0f, num_sms_, 0, invariant_);
     DDNM_CHECK(!Ls.pair && Ls.BN == L.BN, "split-K: tile shape changed");
     Ls.p.split_k = S;
     Ls.p.split_stride = stride;
@@ -183,7 +195,8 @@ void UNetEngine::emit_tc(const std::string& name, const SplitView& a, int mode, 
 }
 
 bool UNetEngine::fused_ok(const View& x, const View* side, int Cout, const View& out) const {
-  return terms_ == 3 && x.st != nullptr && tc_gn_eligible(x, side, Cout, out);
+  // not in batch-invariant mode: the GN form runs DUAL and carries GroupNorm sums across tiles
+  return terms_ == 3 && !invariant_ && x.st != nullptr && tc_gn_eligible(x, side, Cout, out);
 }
 
 void UNetEngine::emit_tcgn(const std::string& name, const View& x, const std::string& norm, const float* ss, int ss_ld, const View* side,
@@ -228,7 +241,8 @@ void UNetEngine::emit_up2_conv(const std::string& name, const SplitView& a, cons
   __half* wl = (__half*)arena_.alloc(4 * per_phase * sizeof(__half));
   presum_up2_weights(P(wname, (long long)Cout * Cin * 9), Cout, Cin, wh, wl, 0);
   for (int ph = 0; ph < 4; ++ph) {
-    TcLaunch L = tc_make_up2_launch(a, wh + ph * per_phase, wl + ph * per_phase, Cout, out, chanadd, ca_ld, ph >> 1, ph & 1, num_sms_);
+    TcLaunch L = tc_make_up2_launch(a, wh + ph * per_phase, wl + ph * per_phase, Cout, out, chanadd, ca_ld, ph >> 1, ph & 1, num_sms_,
+                                     invariant_);
     const double bytes = (double)a.N * a.H * a.W * Cin * 4 + (double)per_phase * 4 + (double)a.N * a.H * a.W * Cout * 4;
     add_op(name + ".ph" + std::to_string(ph), "tc", L.flops, bytes, [L](cudaStream_t s) { tc_run(L, s); });
   }
@@ -267,14 +281,14 @@ void UNetEngine::emit_attention_core(const std::string& name, int T, int heads, 
     const long long hs = head_stride ? head_stride : qkv_ld;   // extent-1 dims still need a legal (non-zero) TMA stride
     GemmOperand A{qh + q_off, ql + q_off, qkv_ld, hs, img};
     GemmOperand Bk{qh + k_off, ql + k_off, qkv_ld, hs, img};
-    TcLaunch L1 = tc_make_gemm_launch(A, Bk, T, T, ch, heads, Bn, S, (long long)heads * T * T, (long long)T * T, T, alpha, num_sms_);
+    TcLaunch L1 = tc_make_gemm_launch(A, Bk, T, T, ch, heads, Bn, S, (long long)heads * T * T, (long long)T * T, T, alpha, num_sms_, invariant_);
     add_op(name + ".qk", "tc", L1.flops, (double)Bn * T * qkv_ld * 4 + sbytes, [L1](cudaStream_t s) { tc_run(L1, s); });
     add_op(name + ".softmax", "softmax", 0, sbytes * 2, [=](cudaStream_t s) { softmax_split(S, (long long)Bn * heads * T, T, ph, pl, s); });
     add_op(name + ".v_transpose", "gn_split", 0, (double)Bn * T * C * 8,
            [=](cudaStream_t s) { transpose_split(q, qkv_ld, head_stride, v_off, Bn, T, heads, ch, vh, vl, s); });
     GemmOperand P{ph, pl, T, (long long)T * T, (long long)heads * T * T};
     GemmOperand Vt{vh, vl, T, (long long)ch * T, (long long)heads * ch * T};
-    TcLaunch L2 = tc_make_gemm_launch(P, Vt, T, ch, T, heads, Bn, O, (long long)T * C, ch, C, 1.0f, num_sms_);
+    TcLaunch L2 = tc_make_gemm_launch(P, Vt, T, ch, T, heads, Bn, O, (long long)T * C, ch, C, 1.0f, num_sms_, invariant_);
     add_op(name + ".pv", "tc", L2.flops, sbytes + (double)Bn * T * C * 8, [L2](cudaStream_t s) { tc_run(L2, s); });
   } else {
     add_op(name + ".qk", "sgemm", fl, (double)Bn * heads * T * (2.0 * ch + T) * 4, [=](cudaStream_t s) {
@@ -353,6 +367,11 @@ void UNetEngine::set_terms(int t) {
   DDNM_CHECK(!finalized_, "precision must be chosen before finalize");
   DDNM_CHECK(t == 1 || t == 3, "terms must be 1 (fast fp16) or 3 (fp32-grade)");
   terms_ = t;
+}
+
+void UNetEngine::set_batch_invariant(bool on) {
+  DDNM_CHECK(!finalized_, "batch-invariant mode must be chosen before finalize");
+  invariant_ = on;
 }
 
 void UNetEngine::finalize() {

@@ -59,6 +59,9 @@ struct OpenAICfg {
   int new_attention_order = 0;   // 1: QKVAttention (q, k, v split before the heads, unet.py:361-389); 0: QKVAttentionLegacy
 };
 
+// tests: engines built after the call size their grids and launch policy for min(n, the device's count) SMs (0 = the device's count)
+void engine_debug_sm_count(int n);
+
 class UNetEngine {
  public:
   UNetEngine(int batch, int in_channels, int out_ch, int resolution, int groups, float eps);
@@ -88,6 +91,9 @@ class UNetEngine {
   void set_use_graph(bool on) { use_graph_ = on; }
   // 3 = fp32-grade products (parity mode, default); 1 = single fp16 product per MAC (fast, NOT parity-grade). Before finalize.
   void set_terms(int t);
+  // batch-invariant mode (see tc_make_launch): every image's result depends on that image and the layer shapes alone, not on the
+  // batch size, the image's row, padding rows or the SM count.  Before finalize.
+  void set_batch_invariant(bool on);
   size_t workspace_bytes() const { return arena_.used(); }
   int num_launches() const { return (int)ops_.size(); }
   double flops_per_forward() const;
@@ -142,6 +148,7 @@ class UNetEngine {
   int num_sms_ = 132;
   bool finalized_ = false, use_graph_ = true;
   int terms_ = 3;
+  bool invariant_ = false;
   Arena arena_;
   std::map<std::string, Param> params_;
   std::vector<OpRecord> ops_;

@@ -595,7 +595,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
       // reduced across the 8 lanes that share a column pair; (2) per image slot: the warps of that image added in a fixed order
       // into running (value, compensation) pairs that persist while consecutive tiles of this CTA stay in the same image and
       // channel block (the tile -> CTA map is static, so these fp32 partial sums are the same every run); (3) flushed with one
-      // order-independent fixed-point add per value otherwise
+      // order-independent fixed-point add per value otherwise, and after every tile with p.stat_per_tile
       tc_stats_rows<BN>(d, part + warp * BN, lane, cq);
       named_bar_sync(1, kConsumerThreads);
       const int nslots = 8 / wpi;
@@ -603,7 +603,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
       if (u + unit_step < unit_end) {
         int nn_idx, nx0, ny0, nn0;
         decode(tile_of(u + unit_step), nn_idx, nx0, ny0, nn0);
-        flush = nslots > 1 || nn0 != n0 || nn_idx != n_idx;
+        flush = p.stat_per_tile || nslots > 1 || nn0 != n0 || nn_idx != n_idx;
       }
       for (int i = tid; i < 2 * BN; i += kConsumerThreads) {
         const int which = i / BN, col = i - which * BN;
@@ -889,7 +889,7 @@ conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid
       const int nslots = 8 / wpi;
       bool flush = true;
       const int un = u + 2 * unit_step;   // this warpgroup's next unit
-      if (un < unit_end) {
+      if (!p.stat_per_tile && un < unit_end) {
         int nn_idx, nx0, ny0, nn0;
         tc_decode(p, un / p.split_k, nn_idx, nx0, ny0, nn0);
         flush = nslots > 1 || nn0 != n0 || nn_idx != n_idx;
@@ -997,7 +997,7 @@ void tc_debug_deal(int mode) {
 
 TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1, const __half* w_hi, const __half* w_lo,
                         int w_batches, int Cout, const View& out, const float* chanadd, int ca_ld, const float* residual,
-                        int ldr, float alpha, int num_sms, int res_mode) {
+                        int ldr, float alpha, int num_sms, int res_mode, bool invariant) {
   TcLaunch L;
   TcParams& p = L.p;
   const int taps = (mode0 == TAPS_1X1) ? 1 : (mode0 == TAPS_UP2X2 ? 4 : 9);
@@ -1027,9 +1027,11 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
   // two waves of tiles and 74.6 ms without — the weight traffic they save is not what limits these layers.
   {
     const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
-    L.pair = g_pair_mode == 1 && w_batches == 1 && m_tiles % 2 == 0;
+    L.pair = !invariant && g_pair_mode == 1 && w_batches == 1 && m_tiles % 2 == 0;
   }
-  L.dual = g_dual_mode != 0 && (!L.pair || g_pair_dual != 0);
+  // batch-invariant launches run the three-instruction form, which conv_tc_kernel without DUAL and the ping-pong kernel share
+  // element for element, so the kernel a launch picks (tc_run: tiles per CTA) cannot change a value
+  L.dual = !invariant && g_dual_mode != 0 && (!L.pair || g_pair_dual != 0);
   L.pingpong = g_pingpong_enable != 0;
   p.mode0 = mode0;
   p.cb0 = src0.C / BK;
@@ -1052,6 +1054,7 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
   p.chanadd = chanadd; p.ca_ld = ca_ld; p.residual = residual; p.ldr = ldr; p.alpha = alpha; p.res_mode = res_mode;
   p.stats = out.st; p.st_ld = out.st_ld;
   p.terms = g_terms;
+  p.stat_per_tile = invariant ? 1 : 0;
   if (out.st) DDNM_CHECK(p.bw * p.bh >= 32, "GroupNorm statistics need >= 32 pixels per image");
   if (residual) DDNM_CHECK(ldr % 2 == 0 && ((uintptr_t)residual & 7) == 0, "residual misaligned (rows move as float2)");
   if (chanadd) DDNM_CHECK(ca_ld % 2 == 0 && ((uintptr_t)chanadd & 7) == 0, "channel-add rows misaligned");
@@ -1104,12 +1107,12 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
 }
 
 TcLaunch tc_make_up2_launch(const SplitView& src, const __half* w_hi, const __half* w_lo, int Cout, const View& out, const float* chanadd,
-                            int ca_ld, int py, int px, int num_sms) {
+                            int ca_ld, int py, int px, int num_sms, bool invariant) {
   DDNM_CHECK(out.H == 2 * src.H && out.W == 2 * src.W && out.N == src.N, "upsample phase: output must be twice the source size");
   View lr = out;   // tile over the low-res pixel grid; every tile pixel (y, x) lands on output pixel (2y+py, 2x+px)
   lr.H = src.H;
   lr.W = src.W;
-  TcLaunch L = tc_make_launch(src, TAPS_UP2X2, nullptr, w_hi, w_lo, 1, Cout, lr, chanadd, ca_ld, nullptr, 0, 1.0f, num_sms, 0);
+  TcLaunch L = tc_make_launch(src, TAPS_UP2X2, nullptr, w_hi, w_lo, 1, Cout, lr, chanadd, ca_ld, nullptr, 0, 1.0f, num_sms, 0, invariant);
   TcParams& p = L.p;
   p.up_py = py;
   p.up_px = px;
@@ -1121,7 +1124,7 @@ TcLaunch tc_make_up2_launch(const SplitView& src, const __half* w_hi, const __ha
 }
 
 TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, int N, int K, int heads, int images, float* out,
-                             long long out_sn, long long out_sy, long long out_sx, float alpha, int num_sms) {
+                             long long out_sn, long long out_sy, long long out_sx, float alpha, int num_sms, bool invariant) {
   TcLaunch L;
   TcParams& p = L.p;
   // K and N need not fill whole 64-wide blocks: the operand maps end at K and N, so TMA zero-fills the rest of the last k-block and
@@ -1134,7 +1137,8 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
   // as for the convolutions: BN = 128 unless it leaves most SMs idle
   L.BN = 64;
   if (N % 128 == 0 && (long long)m_tiles * (N / 128) >= num_sms / 2) L.BN = 128;
-  L.dual = g_dual_mode != 0;
+  if (g_force_bn && N % g_force_bn == 0) L.BN = g_force_bn;   // tests / tuning experiments only
+  L.dual = !invariant && g_dual_mode != 0;   // as in tc_make_launch (no GroupNorm sums here)
   L.pingpong = g_pingpong_enable != 0;
   p.n_tiles = cdiv(N, L.BN);
   L.ntail = N % L.BN != 0;

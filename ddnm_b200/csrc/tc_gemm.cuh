@@ -39,6 +39,8 @@ struct TcParams {
   long long split_stride = 0;  //      (no chanadd / residual / stats: splitk_reduce applies them)
   int deal = 0;                // tile -> CTA map: 0 round-robin, 1 one contiguous range per CTA (see conv_tc_kernel)
   int terms;                   // 3: hi*hi + hi*lo + lo*hi (fp32-grade, default); 1: hi*hi only (plain fp16 inputs, fast mode)
+  int stat_per_tile = 0;       // 1 (batch-invariant launches): each tile's GroupNorm partials go to `stats` on their own, never
+                               //    carried into the CTA's next tile, so their grouping depends only on the tile's place in its image
 };
 
 // GN form (fused GroupNorm + SiLU + split + 3x3 convolution, see conv_tc_kernel): the A operand is produced from fp32 rows
@@ -78,14 +80,16 @@ struct TcLaunch {
 
 // Build the launch record.  src0/src1: fp16 split activations; w_hi/w_lo: [batch][Cout][Ktot] fp16 K-major with
 // Ktot = taps*C0 + C1 (k index = tap*C0 + ci, then source-1 channels).
+// invariant: batch-invariant launch — an output element's arithmetic depends only on its image and the layer's shape, not on
+// the batch, the image's place in it or num_sms (no DUAL form, no CTA pairs of conv_tc_kernel, GroupNorm partials flushed per tile)
 TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1, const __half* w_hi, const __half* w_lo,
                         int w_batches, int Cout, const View& out, const float* chanadd, int ca_ld, const float* residual,
-                        int ldr, float alpha, int num_sms, int res_mode = 0);
+                        int ldr, float alpha, int num_sms, int res_mode = 0, bool invariant = false);
 void tc_run(const TcLaunch& L, cudaStream_t stream);
 // One parity phase (py, px) of conv3x3(nearest_upsample_x2(src)): src is the LOW-res split, w_* the phase's pre-summed
 // [Cout][4*Cin] weights (see presum_up2_weights), out the FULL-res view; writes out[:, 2y+py, 2x+px, :].
 TcLaunch tc_make_up2_launch(const SplitView& src, const __half* w_hi, const __half* w_lo, int Cout, const View& out, const float* chanadd,
-                            int ca_ld, int py, int px, int num_sms);
+                            int ca_ld, int py, int px, int num_sms, bool invariant = false);
 
 // Strided fp16 (hi, lo) operand for the batched-GEMM builder: element (k, row, head, image) at
 // base[k + row*s_row + head*s_head + image*s_img]; k extent = K (multiple of 8; base and strides 16-byte aligned).
@@ -98,7 +102,7 @@ struct GemmOperand {
 // (multi-head attention: QK^T and PV).  M % 128 == 0, N % 8 == 0, K % 8 == 0: a partial last k-block / N tile is zero-filled by
 // TMA, and no column past N is stored.
 TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, int N, int K, int heads, int images, float* out,
-                             long long out_sn, long long out_sy, long long out_sx, float alpha, int num_sms);
+                             long long out_sn, long long out_sy, long long out_sx, float alpha, int num_sms, bool invariant = false);
 
 // ---- fused GroupNorm + SiLU + split + 3x3 convolution (the GN form of conv_tc_kernel) ----
 struct GnAffine {
@@ -118,7 +122,7 @@ TcLaunch tc_make_gn_launch(const View& x, const GnAffine& gn, const View* side, 
 void tc_debug_gn_fused(int on);      // 1: eligible layers of engines built afterwards use the GN form; 0 (default): gn_apply + conv_tc
 
 // debug knobs (tests only): apply to the launches built afterwards
-void tc_debug_force_bn(int bn);      // 0 (default): heuristic, 64 / 128: force the N tile where Cout allows it
+void tc_debug_force_bn(int bn);      // 0 (default): heuristic, 64 / 128: force the N tile where Cout (GEMM: N) allows it
 void tc_debug_deal(int mode);        // -1 (default): contiguous tile ranges where they pay (one N tile + GroupNorm sums), 0 / 1: force
 void tc_debug_pair_mode(int mode);   // -1 (default) / 0: no CTA pairs, 1: CTA pairs wherever legal
 void tc_debug_dual_mode(int mode);   // 1 (default): DUAL form for single-CTA launches, 0: never

@@ -144,7 +144,9 @@ def restore(model, gt, classes, deg="sr_averagepooling", scale=4, sigma_y=0.0, r
     tensor (B,3,H,W) — H, W = gt's size (x scale with ``resize_y``).  ``noise``: optional (n_draws,B,3,256,256) tape in the
     reference's draw order (initial x, then one per p_sample / undo call); by default the draws come from torch's generator in
     that order.  ``seed``: the library draws them instead (stream tag 3, draw index = position in that order, row = image), inside
-    the step kernels; reproducible against itself, not against torch's generator."""
+    the step kernels; reproducible against itself, not against torch's generator.  The row is the image's index within this
+    call (there is no row_offset), so with ``model.batch_invariant`` an image restores bit-identically in any call where it has
+    the same index, e.g. alone and as row 0 of a batch."""
     if seed is not None and noise is not None:
         raise ValueError("seed= and noise= are two sources for the same draws: give one")
     if not isinstance(model, _EngineModel):

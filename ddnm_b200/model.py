@@ -30,6 +30,22 @@ class _EngineModel:
         self.precision = "fp32"
         _lib.lib()              # fail early if the CUDA library is absent
 
+    # True: every image's output is computed by arithmetic that depends only on that image and the layer shapes, not on the batch
+    # size, its row in the batch, padding rows or the GPU's SM count; with seeded noise a restoration is then bit-identical however
+    # it is batched or sharded.  Slower (see DESIGN.md §4).  Applied when an engine is built; changing it drops the built engines.
+    _batch_invariant = False
+
+    @property
+    def batch_invariant(self):
+        return self._batch_invariant
+
+    @batch_invariant.setter
+    def batch_invariant(self, on):
+        on = bool(on)
+        if on != self._batch_invariant:
+            self._destroy()
+        self._batch_invariant = on
+
     def load_state_dict(self, sd, strict=True):
         self._sd = {k.replace("module.", "", 1) if k.startswith("module.") else k: v.detach().float().contiguous()
                     for k, v in sd.items()}
@@ -69,6 +85,7 @@ class _EngineModel:
         if self.precision not in ("fp32", "fp16"):
             raise ValueError("precision must be 'fp32' (parity) or 'fp16' (fast)")
         _lib.check(L.ddnm_unet_set_precision(h, 3 if self.precision == "fp32" else 1))
+        _lib.check(L.ddnm_unet_set_batch_invariant(h, 1 if self.batch_invariant else 0))
         _lib.check(L.ddnm_unet_finalize(h))
         _lib.check(L.ddnm_unet_set_graph(h, 1 if self.use_cuda_graph else 0))
         self._engines[batch] = h

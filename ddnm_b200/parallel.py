@@ -29,8 +29,9 @@ def sharded_sample(sample_fn, x, y, noise=None, group=None):
 
 def sharded_sample_seeded(sample_fn, x, y, seed, group=None):
     """As ``sharded_sample`` with library-drawn noise: runs ``sample_fn(x_rows, y_rows, seed, row_offset=lo)`` on this rank's rows
-    [lo, hi) and all-gathers.  A seeded draw depends on the GLOBAL row index only, so no rank needs a noise tape and the result
-    equals the unsharded ``sample_fn(x, y, seed, row_offset=0)`` row for row, at any world size."""
+    [lo, hi) and all-gathers.  A seeded draw depends on the GLOBAL row index only, so no rank needs a noise tape.  With the
+    model (and classifier) in ``batch_invariant`` mode the result equals the unsharded ``sample_fn(x, y, seed, row_offset=0)``
+    bit for bit, at any world size; otherwise it agrees to fp32 reassociation."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     B = x.shape[0]

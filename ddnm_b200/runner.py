@@ -138,8 +138,9 @@ def restore_batch(config, model, A_funcs, deg, x_orig, betas, eta, sigma_y=0.0, 
     when it is given.
 
     ``seed``: x_T, the ``add_noise`` term and the loop's draws come from the library's seeded generator with
-    ``row_offset = idx_so_far``, so image i of a dataset restores identically whatever ``sampling.batch_size`` is (the
-    dequantisation draws of ``data_transform``, off in every shipped config, stay torch's).
+    ``row_offset = idx_so_far``, so image i of a dataset gets the same draws whatever ``sampling.batch_size`` is (the
+    dequantisation draws of ``data_transform``, off in every shipped config, stay torch's); with ``model.batch_invariant``
+    it restores bit-identically, otherwise to fp32 reassociation.
     """
     dev = torch.device("cuda")
     C_, R = config.data.channels, config.data.image_size

@@ -329,7 +329,8 @@ int ddnm_conv_gn_tc(const float* x, int N, int H, int W, int Cin, int groups, co
 /* 1: eligible layers (3x3, rows >= 128 pixels) of engines built afterwards run the fused GroupNorm convolution; 0 (default, also env
  * DDNM_GN_FUSED): gn_apply_kernel + conv_tc_kernel */
 int ddnm_tc_debug_gn_fused(int on);
-/* tuning experiments: force the N-tile width (64 or 128) of conv launches built afterwards (0 = heuristic) */
+/* tuning experiments: force the N-tile width (64 or 128) of conv and attention-GEMM launches built afterwards where the output
+ * width allows it (0 = heuristic) */
 int ddnm_tc_debug_force_bn(int bn);
 /* tile -> CTA map of conv launches built afterwards: -1 (default) contiguous tile ranges per CTA on layers with one N tile that
  * produce GroupNorm sums, 0 round-robin everywhere, 1 contiguous wherever legal */
@@ -352,6 +353,13 @@ int ddnm_tc_debug_pingpong(int on);
 /* 1 (default, also env DDNM_PP_PAIR): ping-pong launches (not the upsample phases), built afterwards, run on clusters of two CTAs that each
  * load half of every weight k-block and multicast it to both (bit-identical output); 0: single CTAs */
 int ddnm_tc_debug_pp_pair(int on);
+/* Batch-invariant mode, chosen before finalize on a UNet, SuperRes or classifier handle (default 0).  1: every image's forward
+ * (and the classifier's input gradient) is computed by arithmetic that depends only on that image and the layer shapes, not on the
+ * batch size, the image's row, padding rows or the SM count, so a seeded restoration is bit-identical however it is batched or
+ * sharded.  Costs throughput (no DUAL form, GroupNorm partials flushed per tile, split-K by the per-image shape). */
+int ddnm_unet_set_batch_invariant(void* handle, int on);
+/* tests: engines created afterwards size their grids and launch policy for min(n, the device's count) SMs; 0 = the device's count */
+int ddnm_tc_debug_sm_count(int n);
 
 #ifdef __cplusplus
 }
