@@ -125,13 +125,9 @@ _SIGS = {
     "ddnm_conv_tc_bench": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, C.POINTER(_F), C.POINTER(_D)]),
     "ddnm_gnconv_chunk_bench": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, C.POINTER(_F)]),
     "ddnm_groupnorm": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, _F, _I, _P, _P]),
-    "ddnm_conv_gn_tc": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P, _F, _I, _P, _P, _I, _P, _I, _P, _P, _P, _I, C.POINTER(_F), _P]),
-    "ddnm_tc_debug_gn_fused": (C.c_int, [_I]),
     "ddnm_tc_debug_force_bn": (C.c_int, [_I]),
     "ddnm_tc_debug_deal": (C.c_int, [_I]),
-    "ddnm_tc_debug_pair_dual": (C.c_int, [_I]),
     "ddnm_tc_debug_dual_mode": (C.c_int, [_I]),
-    "ddnm_tc_debug_pair_mode": (C.c_int, [_I]),
     "ddnm_tc_debug_halo": (C.c_int, [_I]),
     "ddnm_tc_debug_pingpong": (C.c_int, [_I]),
     "ddnm_tc_debug_pp_pair": (C.c_int, [_I]),

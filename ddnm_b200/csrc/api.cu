@@ -461,73 +461,14 @@ int ddnm_groupnorm(const float* x, int N, int H, int W, int C, int groups, const
   DDNM_API_END
 }
 
-// out = conv3x3(silu?(groupnorm(x))) [+ conv1x1(side_x)] + bias [+ residual] through the fused GN form of the convolution kernel;
-// gamma == NULL skips the normalisation.  iters > 0: also time `iters` launches (ms_per_iter may be NULL otherwise).
-int ddnm_conv_gn_tc(const float* x, int N, int H, int W, int Cin, int groups, const float* gamma, const float* beta, float eps, int silu,
-                    const float* w, const float* bias, int Cout, const float* side_x, int CinSide, const float* side_w,
-                    const float* residual, float* out, int iters, float* ms_per_iter, void* stream) {
-  DDNM_API_BEGIN
-  cudaStream_t s = (cudaStream_t)stream;
-  Tmp tmp;
-  View xv = mkview(const_cast<float*>(x), N, H, W, Cin);
-  StatAcc* st = tmp.get<StatAcc>((size_t)N * Cin * 2);
-  CUDA_CHECK(cudaMemsetAsync(st, 0, (size_t)N * Cin * 2 * sizeof(StatAcc), s));
-  xv.st = st;
-  xv.st_ld = Cin;
-  if (gamma) gn_stats(xv, s);
-  View sv;
-  if (side_x) sv = mkview(const_cast<float*>(side_x), N, H, W, CinSide);
-  const int ktot = 9 * Cin + (side_x ? CinSide : 0);
-  __half* wh = tmp.get<__half>((size_t)Cout * ktot);
-  __half* wl = tmp.get<__half>((size_t)Cout * ktot);
-  split_conv_weight(w, Cout, Cin, 9, wh, wl, ktot, 0, s);
-  if (side_x) split_conv_weight(side_w, Cout, CinSide, 1, wh, wl, ktot, 9 * Cin, s);
-  GnAffine gn;
-  gn.gamma = gamma; gn.beta = beta; gn.eps = eps; gn.groups = groups; gn.silu = silu != 0;
-  View ov = mkview(out, N, H, W, Cout);
-  TcLaunch L = tc_make_gn_launch(xv, gn, side_x ? &sv : nullptr, wh, wl, Cout, ov, bias, 0, residual, Cout, sm_count());
-  tc_run(L, s);
-  if (iters > 0 && ms_per_iter) {
-    cudaEvent_t e0, e1;
-    CUDA_CHECK(cudaEventCreate(&e0));
-    CUDA_CHECK(cudaEventCreate(&e1));
-    for (int i = 0; i < 2; ++i) tc_run(L, s);
-    CUDA_CHECK(cudaEventRecord(e0, s));
-    for (int i = 0; i < iters; ++i) tc_run(L, s);
-    CUDA_CHECK(cudaEventRecord(e1, s));
-    CUDA_CHECK(cudaEventSynchronize(e1));
-    float ms = 0;
-    CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    *ms_per_iter = ms / iters;
-  }
-  CUDA_CHECK(cudaStreamSynchronize(s));
-  DDNM_API_END
-}
-int ddnm_tc_debug_gn_fused(int on) {
-  DDNM_API_BEGIN
-  tc_debug_gn_fused(on);
-  DDNM_API_END
-}
 int ddnm_tc_debug_deal(int mode) {
   DDNM_API_BEGIN
   tc_debug_deal(mode);
   DDNM_API_END
 }
-int ddnm_tc_debug_pair_mode(int mode) {
-  DDNM_API_BEGIN
-  tc_debug_pair_mode(mode);
-  DDNM_API_END
-}
 int ddnm_tc_debug_dual_mode(int mode) {
   DDNM_API_BEGIN
   tc_debug_dual_mode(mode);
-  DDNM_API_END
-}
-int ddnm_tc_debug_pair_dual(int on) {
-  DDNM_API_BEGIN
-  tc_debug_pair_dual(on);
   DDNM_API_END
 }
 int ddnm_tc_debug_halo(int on) {

@@ -169,7 +169,7 @@ void UNetEngine::emit_tc(const std::string& name, const SplitView& a, int mode, 
   const int tiles = L.p.tiles_x * L.p.tiles_y * L.p.tiles_n * L.p.n_tiles, kblocks = L.p.kb0 + L.p.kb1;
   static const bool split_on = std::getenv("DDNM_SPLITK") == nullptr || std::atoi(std::getenv("DDNM_SPLITK")) != 0;
   int S = 1;
-  if (split_on && !L.pair && res_mode == 0 && kblocks >= 32) {
+  if (split_on && res_mode == 0 && kblocks >= 32) {
     // batch-invariant mode: S is part of an element's arithmetic (the k-block ranges and their fixed-order sum), so it follows the
     // per-image shape alone — 2 on the maps of at most 64 pixels, the 8x8 level where B = 16 splits by the tile count as well
     if (invariant_) S = out.H * out.W <= 64 ? 2 : 1;
@@ -181,7 +181,7 @@ void UNetEngine::emit_tc(const std::string& name, const SplitView& a, int mode, 
     View pv;
     pv.p = part; pv.N = out.N; pv.H = out.H; pv.W = out.W; pv.C = Cout; pv.ld = Cout;
     TcLaunch Ls = tc_make_launch(a, mode, side, w.hi, w.lo, 1, Cout, pv, nullptr, 0, nullptr, 0, 1.0f, num_sms_, 0, invariant_);
-    DDNM_CHECK(!Ls.pair && Ls.BN == L.BN, "split-K: tile shape changed");
+    DDNM_CHECK(Ls.BN == L.BN, "split-K: tile shape changed");
     Ls.p.split_k = S;
     Ls.p.split_stride = stride;
     Ls.halo = false;   // k-block ranges of a split need not be whole A units
@@ -191,28 +191,6 @@ void UNetEngine::emit_tc(const std::string& name, const SplitView& a, int mode, 
            [=](cudaStream_t s) { splitk_reduce(part, S, stride, out, chanadd, ca_ld, residual, ldr, s); });
     return;
   }
-  add_op(name, "tc", L.flops, bytes, [L](cudaStream_t s) { tc_run(L, s); });
-}
-
-bool UNetEngine::fused_ok(const View& x, const View* side, int Cout, const View& out) const {
-  // not in batch-invariant mode: the GN form runs DUAL and carries GroupNorm sums across tiles
-  return terms_ == 3 && !invariant_ && x.st != nullptr && tc_gn_eligible(x, side, Cout, out);
-}
-
-void UNetEngine::emit_tcgn(const std::string& name, const View& x, const std::string& norm, const float* ss, int ss_ld, const View* side,
-                           const TcWeights& w, int Cout, const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr) {
-  GnAffine gn;
-  gn.gamma = P(norm + ".weight", x.C);
-  gn.beta = P(norm + ".bias", x.C);
-  gn.eps = eps_;
-  gn.groups = groups_;
-  gn.silu = true;
-  gn.ss = ss;
-  gn.ss_ld = ss_ld;
-  TcLaunch L = tc_make_gn_launch(x, gn, side, w.hi, w.lo, Cout, out, chanadd, ca_ld, residual, ldr, num_sms_);
-  // algorithmic HBM bytes: the fp32 activation(s) in, the weights, the fp32 output (+ residual) — no fp16 planes
-  const double bytes = (double)x.pixels() * x.C * 4 + (side ? (double)side->pixels() * side->C * 4 : 0) + (double)Cout * w.ktot * 4 +
-                       (double)out.pixels() * Cout * 4 * (residual ? 2 : 1);
   add_op(name, "tc", L.flops, bytes, [L](cudaStream_t s) { tc_run(L, s); });
 }
 

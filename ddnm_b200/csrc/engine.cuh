@@ -118,11 +118,6 @@ class UNetEngine {
                      const float* ss = nullptr, int ss_ld = 0, SplitView* raw = nullptr);
   void emit_tc(const std::string& name, const SplitView& a, int mode, const SplitView* side, const TcWeights& w, int Cout,
                const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int res_mode = 0);
-  // fused form of emit_gn_split + emit_tc for 3x3 convolutions on rows >= 128 pixels wide (the GN form of conv_tc_kernel): x is
-  // normalised (norm = parameter prefix), activated, split and convolved in one kernel; side = raw fp32 input of a 1x1 shortcut
-  bool fused_ok(const View& x, const View* side, int Cout, const View& out) const;
-  void emit_tcgn(const std::string& name, const View& x, const std::string& norm, const float* ss, int ss_ld, const View* side,
-                 const TcWeights& w, int Cout, const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr);
   // softmax(alpha * Q K^T) V for `heads` heads of width ch over T tokens; q/k/v live in the fp32 qkv_ buffer
   // ([token][qkv_ld], head h at column h*head_stride + {q_off, k_off, v_off}); result -> attO_ [token][heads*ch].
   // T % 128 == 0 and ch % 8 == 0 run both contractions on the tensor cores (a head width that is not a multiple of 64 ends in a

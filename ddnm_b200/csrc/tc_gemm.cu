@@ -20,10 +20,6 @@
 //         a single m64 x 2BN instruction (accumulator columns [0, BN) = hi*hi, [BN, 2BN) = hi*lo); A_lo x B_hi follows with N = BN
 //         into the first half, and the epilogue adds the halves: two instructions and one read of the A_hi rows per k-step
 //         instead of three and two.
-//   PAIR: a cluster of two CTAs works on two M-adjacent tiles with the same N tile; each CTA TMA-loads its own A tile and HALF of
-//         the B tile, multicast into both CTAs' shared memory, so every weight row crosses L2 -> SM once per pair instead of twice.
-//         A stage may be refilled only when the consumers of BOTH CTAs have released it: each empty barrier counts the arrivals of
-//         the 16 consumer warps of the cluster.
 //   HALO: 3x3 stride-1 and upsample-phase (2x2) launches whose tile rows are 64-pixel runs of image rows (bw % 64 == 0, one image
 //         per tile).  The three column taps dx of a (dy, 64-channel slice) read the same image rows shifted by one pixel, so the
 //         producer loads them once, as a halo unit of (bw + 2) x bh pixels (bw + 1 for the upsample phases) in hi + lo, and the
@@ -33,14 +29,9 @@
 //         A units have a ring of their own (HALO_UNITS, own full / empty barriers) next to a ring of 4 B stages; a unit goes back to
 //         the producer once the wgmma group of its last dx k-block has completed.  Launches with a 1x1 side input keep the per-tap
 //         form (see tc_make_launch).
-// And one with another A operand:
-//   GN:   fused GroupNorm + SiLU + fp16 split + 3x3 convolution (+ 1x1 shortcut as extra K blocks) on rows of >= 128 pixels.  Each
-//         consumer warpgroup reads its 64 pixels of the shifted fp32 rows itself, applies the per-(image, channel) affine of the
-//         normalisation (from the producer-side GroupNorm sums, plus scale-shift), SiLU, splits to fp16 hi / lo and stores them in
-//         the 128B-swizzled K-major layout TMA would have written; `fence.proxy.async` makes the generic-proxy stores visible to
-//         its wgmma.  The producer loads only the weights.  The fp16 planes of the activation never exist in HBM.
-// conv_tc_pingpong_kernel (below) runs the single-CTA launches without GN where CTAs walk several tiles: each consumer warpgroup
-// owns a whole tile, and the two take turns on the tensor cores so one tile's epilogue overlaps the next tile's MMAs.
+// conv_tc_pingpong_kernel (below) runs the launches where CTAs walk several tiles: each consumer warpgroup owns a whole tile, and
+// the two take turns on the tensor cores so one tile's epilogue overlaps the next tile's MMAs.  Its launches with one weight matrix
+// run on clusters of two CTAs that share every weight k-block through TMA multicast (its PAIR form).
 #include "tc_gemm.cuh"
 
 #include <cstdlib>
@@ -52,7 +43,6 @@ static constexpr int kConsumerThreads = 256;
 static constexpr int kTcThreads = kConsumerThreads + 32;
 static constexpr int BK = 64;                      // fp16 elements = 128 bytes = one swizzle row
 static constexpr int A_PLANE_BYTES = BM * BK * 2;  // 16 KiB
-static constexpr int kGnMaxC = 512;                // GN form: widest normalised input
 
 // HALO form: one A plane of a unit holds the halo rows of a tile, (bw + 2) x bh pixels of 128 B (at most 132 rows), 1024 B-aligned.
 // 2 units + 4 B stages: one unit feeds 3 (2) k-blocks, so the A ring still runs as far ahead as the B ring; celeba forward (B = 16,
@@ -73,8 +63,7 @@ struct TcCfg {
   // of up to 4 images per tile x {sum, sumsq} x BN columns
   static constexpr int PART_BYTES = 8 * BN * 8;
   static constexpr int RUN_BYTES = 4 * 2 * BN * 8;
-  static constexpr int GN_BYTES = 2 * kGnMaxC * 4;   // GN form: per-channel scale and shift of the tile's image
-  static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + PART_BYTES + RUN_BYTES + GN_BYTES;
+  static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + PART_BYTES + RUN_BYTES;
   static constexpr int ACC = DUAL ? BN : BN / 2;     // fp32 accumulator registers per consumer thread (m64 x BN(x2) / 128 threads)
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory capacity");
 };
@@ -87,22 +76,6 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[R], uint64_t a, uint64_t b
   if constexpr (N == 64) wgmma_m64n64k16(*reinterpret_cast<float(*)[32]>(&d[0]), a, b, accumulate);
   else if constexpr (N == 128) wgmma_m64n128k16(*reinterpret_cast<float(*)[64]>(&d[0]), a, b, accumulate);
   else wgmma_m64n256k16(*reinterpret_cast<float(*)[128]>(&d[0]), a, b, accumulate);
-}
-
-// GN form: 32 consecutive channels of one pixel (normalised + activated, or raw) -> fp16 hi / lo, stored as 4 swizzled 16-byte chunks
-// of row `row` (0..127) of the two 128-row A planes at a_hi / a_hi + A_PLANE_BYTES
-__device__ __forceinline__ void gn_store_row(uint8_t* a_hi, int row, int chunk0, const float (&v)[32]) {
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    uint4 h, l;
-    split2_f16(v[8 * q + 0], v[8 * q + 1], h.x, l.x);
-    split2_f16(v[8 * q + 2], v[8 * q + 3], h.y, l.y);
-    split2_f16(v[8 * q + 4], v[8 * q + 5], h.z, l.z);
-    split2_f16(v[8 * q + 6], v[8 * q + 7], h.w, l.w);
-    const int off = row * 128 + (((chunk0 + q) ^ (row & 7)) << 4);   // 128B swizzle: 16-byte chunk ^ (row mod 8)
-    *reinterpret_cast<uint4*>(a_hi + off) = h;
-    *reinterpret_cast<uint4*>(a_hi + A_PLANE_BYTES + off) = l;
-  }
 }
 
 // output tile -> (N tile, first column, first row, first image of the M tile)
@@ -137,10 +110,10 @@ struct TcRing {
 
 // TMA loads of the k-blocks [kb_lo, kb_hi) of one output tile, issued by one thread: per k-block the B planes into the next stage
 // and the A operand — the tap-shifted window (3x3, stride-2 phase, upsample phase), the 1x1 side input, or (HALO) one halo unit
-// per (dy, channel slice) at its first dx k-block.  GN: only the B planes (the consumers write A).  PAIR: this CTA's half of the B
-// tile, multicast into both CTAs of the pair.  load_a == false (PAIR only): the B halves alone, in the k order of `tile`, for a peer
-// CTA that has one unit more than this one.
-template <class Cfg, bool PAIR, bool GN, bool HALO>
+// per (dy, channel slice) at its first dx k-block.  PAIR (the ping-pong CTA pairs): this CTA's half of the B tile, multicast into
+// both CTAs of the cluster.  load_a == false (PAIR only, a ghost step): the B halves alone, in the k order of `tile`, for a peer CTA
+// that has one unit more than this one.
+template <class Cfg, bool PAIR, bool HALO>
 __device__ __forceinline__ void tc_produce_tile(const CUtensorMap* tm_a0h, const CUtensorMap* tm_a0l, const CUtensorMap* tm_a1h,
                                                 const CUtensorMap* tm_a1l, const CUtensorMap* tm_bh, const CUtensorMap* tm_bl,
                                                 const TcParams& p, uint32_t smem_base, TcBars<Cfg::STAGES> bars, int tile, int kb_lo,
@@ -149,9 +122,8 @@ __device__ __forceinline__ void tc_produce_tile(const CUtensorMap* tm_a0h, const
   const int halo_w = p.bw + halo_r - 1;
   const bool lo = p.terms != 1;
   const uint32_t planes = lo ? 2u : 1u;
-  // GN / HALO: only the B planes arrive with a stage (GN: the consumers write A themselves)
-  const uint32_t stage_tx = (GN || HALO || !load_a) ? planes * Cfg::B_PLANE_BYTES
-                                                    : (uint32_t)(lo ? Cfg::STAGE_BYTES : Cfg::STAGE_BYTES / 2);
+  // HALO: only the B planes arrive with a stage
+  const uint32_t stage_tx = (HALO || !load_a) ? planes * Cfg::B_PLANE_BYTES : (uint32_t)(lo ? Cfg::STAGE_BYTES : Cfg::STAGE_BYTES / 2);
   int n_idx, x0, y0, n0;
   tc_decode(p, tile, n_idx, x0, y0, n0);
   const int bz = p.b_batched == 1 ? n0 : 0;
@@ -183,7 +155,7 @@ __device__ __forceinline__ void tc_produce_tile(const CUtensorMap* tm_a0h, const
     const uint32_t sb = HALO ? sa : sa + 2 * A_PLANE_BYTES;
     const uint32_t fb = bars.full(r.stage);
     mbar_expect_tx(fb, stage_tx);
-    if (GN || HALO || !load_a) {
+    if (HALO || !load_a) {
     } else if (kb < p.kb0) {
       const int tap = kb / p.cb0;
       const int c = (kb - tap * p.cb0) * BK;
@@ -322,14 +294,11 @@ __device__ __forceinline__ void tc_stats_rows(const float (&d)[R], float2* part,
   }
 }
 
-template <int BN, bool PAIR, bool DUAL, bool GN, bool HALO, bool NTAIL>
+template <int BN, bool DUAL, bool HALO, bool NTAIL>
 __global__ void __launch_bounds__(kTcThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant__ CUtensorMap tm_a0l,
                const __grid_constant__ CUtensorMap tm_a1h, const __grid_constant__ CUtensorMap tm_a1l,
-               const __grid_constant__ CUtensorMap tm_bh, const __grid_constant__ CUtensorMap tm_bl, const TcParams p,
-               const TcGnArgs g) {
-  static_assert(!GN || !PAIR, "the GN form runs on single CTAs");
-  static_assert(!HALO || (!PAIR && !GN), "the HALO form runs on single CTAs with TMA-loaded A");
+               const __grid_constant__ CUtensorMap tm_bh, const __grid_constant__ CUtensorMap tm_bl, const TcParams p) {
   using Cfg = TcCfg<BN, DUAL, HALO>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -346,8 +315,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
   uint8_t* stat_smem = smem_raw + (bar_base + 256u - smem_u32(smem_raw));
   float2* part = reinterpret_cast<float2*>(stat_smem);                    // [warp][BN] {sum, sumsq} over the warp's 16 rows
   float2* run = reinterpret_cast<float2*>(stat_smem + Cfg::PART_BYTES);   // [image slot][which][BN] {value, compensation}
-  float* gn_sc = reinterpret_cast<float*>(stat_smem + Cfg::PART_BYTES + Cfg::RUN_BYTES);   // GN: scale[kGnMaxC], shift[kGnMaxC]
-  float* gn_sh = gn_sc + kGnMaxC;
 
   pdl_prologue();
   const int warp = threadIdx.x >> 5;
@@ -363,37 +330,27 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
   // latency-bound): p.split_k CTAs share a tile, each accumulates its own range of k-blocks and writes alpha * acc to its own
   // partial buffer (p.out + ks * p.split_stride); splitk_reduce_kernel adds the partials in a fixed order, applies the epilogue
   // terms and accumulates the GroupNorm sums — deterministic, no floating-point atomics
-  // PAIR: the scheduling unit is a pair of M-adjacent tiles sharing one N tile; CTA `rank` of the cluster owns tile 2 * mp + rank.
-  // Both CTAs walk the same units (each one's B halves feed the other).
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const int n_units = PAIR ? total_tiles / 2 : total_tiles * p.split_k;
-  const int n_workers = PAIR ? (int)(gridDim.x / 2) : (int)gridDim.x;
-  const int worker = PAIR ? (int)cluster_id_x() : (int)blockIdx.x;
+  const int n_units = total_tiles * p.split_k;
+  const int n_workers = (int)gridDim.x;
+  const int worker = (int)blockIdx.x;
   const int unit_begin = p.deal ? (int)((long long)worker * n_units / n_workers) : worker;
   const int unit_end = p.deal ? (int)((long long)(worker + 1) * n_units / n_workers) : n_units;
   const int unit_step = p.deal ? 1 : n_workers;
   auto k_lo = [&](int u) { return (int)((long long)(u % p.split_k) * KB / p.split_k); };
   auto k_hi = [&](int u) { return (int)((long long)(u % p.split_k + 1) * KB / p.split_k); };
-  auto tile_of = [&](int u) {
-    if (!PAIR) return u / p.split_k;
-    const int mp = u / p.n_tiles;
-    return (2 * mp + (int)rank) * p.n_tiles + (u - mp * p.n_tiles);
-  };
 
   if (warp == 8 && lane == 0) {
-    if (!GN) {
-      tma_prefetch_desc(&tm_a0h);
-      tma_prefetch_desc(&tm_a0l);
-    }
+    tma_prefetch_desc(&tm_a0h);
+    tma_prefetch_desc(&tm_a0l);
     tma_prefetch_desc(&tm_bh);
     tma_prefetch_desc(&tm_bl);
-    if (p.kb1 && !GN) {
+    if (p.kb1) {
       tma_prefetch_desc(&tm_a1h);
       tma_prefetch_desc(&tm_a1l);
     }
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);    // the producer's expect_tx arrive
-      mbar_init(empty_bar(s), PAIR ? 16 : 8);   // one arrive per consumer warp (of both CTAs of a pair)
+      mbar_init(empty_bar(s), 8);   // one arrive per consumer warp
     }
     if (HALO) {
       for (int u = 0; u < HALO_UNITS; ++u) {
@@ -403,8 +360,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
     }
     mbar_fence_init();
   }
-  if (PAIR) cluster_sync_all();   // the peer's barriers exist before any multicast or remote arrive can reach them
-  else __syncthreads();
+  __syncthreads();
 
   auto decode = [&](int tile, int& n_idx, int& x0, int& y0, int& n0) { tc_decode(p, tile, n_idx, x0, y0, n0); };
 
@@ -413,8 +369,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
     if (lane == 0) {
       TcRing ring;
       for (int u = unit_begin; u < unit_end; u += unit_step)
-        tc_produce_tile<Cfg, PAIR, GN, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars, tile_of(u), k_lo(u),
-                                             k_hi(u), rank, ring);
+        tc_produce_tile<Cfg, false, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars, u / p.split_k, k_lo(u),
+                                          k_hi(u), 0u, ring);
     }
   } else {
   // ------------------------------------------------ consumers: wgmma + epilogue ------------------------------------------------
@@ -436,12 +392,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
   }
   float d[Cfg::ACC];
   const bool dual = DUAL && p.terms != 1;
-  int gn_image = -1;   // GN: image whose scale / shift are in gn_sc / gn_sh
   auto release = [&](int s) {
-    if (lane == 0) {
-      mbar_arrive(empty_bar(s));
-      if (PAIR) mbar_arrive_cluster(empty_bar(s), rank ^ 1u);
-    }
+    if (lane == 0) mbar_arrive(empty_bar(s));
   };
   auto release_a = [&](int a) {
     if (lane == 0) mbar_arrive(a_empty_bar(a));
@@ -449,39 +401,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
   for (int u = unit_begin; u < unit_end; u += unit_step) {
     const int kb_lo = k_lo(u), kb_hi = k_hi(u);
     int prev = -1;
-    int t_nidx, t_x0, t_y0, t_n0;   // this tile's coordinates (GN: pixels of the A rows)
-    decode(tile_of(u), t_nidx, t_x0, t_y0, t_n0);
-    if constexpr (GN) {
-      if (g.norm && t_n0 != gn_image && t_n0 < p.N) {
-        // per-channel affine of this image's normalisation, as gn_apply_kernel computes it (double sums, rstd in fp32)
-        named_bar_sync(1, kConsumerThreads);   // both warpgroups are done with the previous image's table
-        const int cpg = g.C / g.groups;
-        const double cnt = (double)p.H * p.W * cpg;
-        for (int c = tid; c < g.C; c += kConsumerThreads) {
-          const int g0 = (c / cpg) * cpg;
-          double s1 = 0, s2 = 0;
-          for (int j = 0; j < cpg; ++j) {
-            s1 += stat_value(g.st[((size_t)t_n0 * g.st_ld + g0 + j) * 2]);
-            s2 += stat_value(g.st[((size_t)t_n0 * g.st_ld + g0 + j) * 2 + 1]);
-          }
-          const double mean = s1 / cnt;
-          double var = s2 / cnt - mean * mean;
-          var = var < 0 ? 0 : var;
-          const float rstd = (float)(1.0 / sqrt(var + (double)g.eps));
-          float a = rstd * g.gamma[c];
-          float b = g.beta[c] - (float)mean * a;
-          if (g.ss) {  // h = norm(h) * (1 + scale) + shift
-            const float one_plus = 1.0f + g.ss[(size_t)t_n0 * g.ss_ld + c];
-            a *= one_plus;
-            b = fmaf(b, one_plus, g.ss[(size_t)t_n0 * g.ss_ld + g.C + c]);
-          }
-          gn_sc[c] = a;
-          gn_sh[c] = b;
-        }
-        named_bar_sync(1, kConsumerThreads);
-        gn_image = t_n0;
-      }
-    }
     for (int kb = kb_lo; kb < kb_hi; ++kb) {
       uint32_t a_base = smem_base + stage * Cfg::STAGE_BYTES + a_row_off;   // this warpgroup's rows of the A_hi plane
       uint32_t a_plane = A_PLANE_BYTES;                                     // A_hi -> A_lo
@@ -505,48 +424,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
       mbar_wait(full_bar(stage), phase);
       const uint32_t sa = smem_base + Cfg::A_RING_BYTES + stage * Cfg::STAGE_BYTES;
       const uint32_t sb = HALO ? sa : sa + 2 * A_PLANE_BYTES;
-      if constexpr (GN) {
-        // this warpgroup's 64 A rows: pixel x0 + row of row y0 (tiles are 128 pixels of one row), shifted by the tap
-        const int rr = (tid & 127) >> 1, half = tid & 1, row = wg * 64 + rr;
-        float v[32];
-        bool valid = t_n0 < p.N;
-        const float* src;
-        if (kb < p.kb0) {
-          const int tap = kb / p.cb0, c0 = (kb - tap * p.cb0) * BK + half * 32;
-          const int yy = t_y0 + tap / 3 - 1, xx = t_x0 + row + tap % 3 - 1;
-          valid = valid && yy >= 0 && yy < p.H && xx >= 0 && xx < p.W;
-          src = g.x + (((long long)t_n0 * p.H + yy) * p.W + xx) * g.x_ld + c0;
-          if (valid) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 f = __ldg(reinterpret_cast<const float4*>(src + 4 * q));
-              v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
-            }
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              if (g.norm) v[j] = fmaf(v[j], gn_sc[c0 + j], gn_sh[c0 + j]);
-              if (g.silu) v[j] = swishf_fast(v[j]);
-            }
-          }
-        } else {   // the 1x1 shortcut's raw input at the output pixel
-          const int c0 = (kb - p.kb0) * BK + half * 32;
-          src = g.xs + (((long long)t_n0 * p.H + t_y0) * p.W + t_x0 + row) * g.xs_ld + c0;
-          if (valid) {
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const float4 f = __ldg(reinterpret_cast<const float4*>(src + 4 * q));
-              v[4 * q] = f.x; v[4 * q + 1] = f.y; v[4 * q + 2] = f.z; v[4 * q + 3] = f.w;
-            }
-          }
-        }
-        if (!valid) {   // the convolution's zero padding (of the activated tensor) and rows past the batch
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = 0.f;
-        }
-        gn_store_row(smem_raw + (sa - smem_u32(smem_raw)), row, half * 4, v);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to wgmma
-        named_bar_sync(2 + wg, 128);
-      }
       const uint64_t ah = wgmma_desc_sw128(a_base);
       const uint64_t al = wgmma_desc_sw128(a_base + a_plane);
       const uint64_t bh = wgmma_desc_sw128(sb);
@@ -588,8 +465,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
 
     // ---- epilogue: rows r0 and r0 + 8 of this tile, 2 adjacent columns per 8-column group ----
     int n_idx, x0, y0, n0;
-    decode(tile_of(u), n_idx, x0, y0, n0);
-    tc_epilogue_rows<BN, DUAL, NTAIL>(p, d, dual, r0, cq, n_idx, x0, y0, n0, PAIR ? 0 : u % p.split_k);
+    decode(u / p.split_k, n_idx, x0, y0, n0);
+    tc_epilogue_rows<BN, DUAL, NTAIL>(p, d, dual, r0, cq, n_idx, x0, y0, n0, u % p.split_k);
     if (p.stats) {
       // GroupNorm statistics of the tile.  (1) per warp: the column sums over its 16 rows (one image: >= 32 pixels per image),
       // reduced across the 8 lanes that share a column pair; (2) per image slot: the warps of that image added in a fixed order
@@ -602,7 +479,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
       bool flush = true;
       if (u + unit_step < unit_end) {
         int nn_idx, nx0, ny0, nn0;
-        decode(tile_of(u + unit_step), nn_idx, nx0, ny0, nn0);
+        decode((u + unit_step) / p.split_k, nn_idx, nx0, ny0, nn0);
         flush = p.stat_per_tile || nslots > 1 || nn0 != n0 || nn_idx != n_idx;
       }
       for (int i = tid; i < 2 * BN; i += kConsumerThreads) {
@@ -628,8 +505,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
     }
   }
   }
-  __syncwarp();                   // the producer warp's lane 0 leaves its loop before the aligned cluster barrier
-  if (PAIR) cluster_sync_all();   // no multicast or remote arrive may reach a CTA that has exited
 }
 
 // -------------------------------------------------------------------------------------------------------------------
@@ -639,7 +514,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid_constant
 // tile order.  A warpgroup hands the turn over right after issuing its last k-block, then waits for its MMAs, releases the stages
 // and runs the epilogue while the other warpgroup's MMAs keep the tensor cores busy.  Each output element gets the products of the
 // three-instruction form in the same order (hi*hi, hi*lo, lo*hi per 16-deep k-step), so the output is bit-identical to
-// conv_tc_kernel without DUAL.  Used for the single-CTA launches without the GN form where a CTA walks at least two tiles.
+// conv_tc_kernel without DUAL.  Used for the launches where a CTA walks at least two tiles (see tc_run).
 // PAIR: clusters of two CTAs.  Each producer loads its own A and HALF of every B k-block, multicast into both CTAs, so a weight row
 // crosses L2 -> SM once per two tiles; a B stage's empty barrier counts the 4 warps of consumer c in this CTA and the 4 of consumer c
 // in the peer.  The tile -> worker deal is the unpaired one; the CTAs of cluster k act as workers w and w + T (T = n_tiles, see
@@ -736,8 +611,8 @@ conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid
     if (threadIdx.x == 0) {
       TcRing ring;
       for (int u = unit_begin; u < unit_end; u += unit_step)
-        tc_produce_tile<Ring, PAIR, false, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars,
-                                                 u / p.split_k, k_lo(u), k_hi(u), PAIR ? cluster_ctarank() : 0u, ring);
+        tc_produce_tile<Ring, PAIR, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars, u / p.split_k,
+                                          k_lo(u), k_hi(u), PAIR ? cluster_ctarank() : 0u, ring);
       if constexpr (PAIR) {
         const int peer_begin = p.deal ? (int)((long long)peer * n_units / n_workers) : peer;
         // ghost steps (the peer has a unit more): this thread fills each stage with its B halves (in the peer tile's k order) and
@@ -755,8 +630,8 @@ conv_tc_pingpong_kernel(const __grid_constant__ CUtensorMap tm_a0h, const __grid
         for (int j = units_of(worker); j < units_of(peer); ++j) {
           for (int kb = 0; kb < KB; ++kb, ++q) {
             if (q >= g0 + STAGES) ghost_release(q - STAGES);
-            tc_produce_tile<Ring, true, false, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars,
-                                                     peer_begin + j * unit_step, kb, kb + 1, cluster_ctarank(), ring, false);
+            tc_produce_tile<Ring, true, HALO>(&tm_a0h, &tm_a0l, &tm_a1h, &tm_a1l, &tm_bh, &tm_bl, p, smem_base, bars,
+                                              peer_begin + j * unit_step, kb, kb + 1, cluster_ctarank(), ring, false);
           }
         }
         for (uint32_t g = q >= g0 + STAGES ? q - STAGES : g0; g < q; ++g) ghost_release(g);
@@ -970,19 +845,12 @@ void tc_debug_force_bn(int bn) {
   DDNM_CHECK(bn == 0 || bn == 64 || bn == 128, "BN must be 0 (heuristic), 64 or 128");
   g_force_bn = bn;
 }
-static int g_pair_mode = -1;   // -1: default (no pairs, see tc_make_launch), 0: never, 1: CTA pairs wherever legal
-void tc_debug_pair_mode(int mode) {
-  DDNM_CHECK(mode == -1 || mode == 0 || mode == 1, "pair mode must be -1 (default rule), 0 (off) or 1 (wherever legal)");
-  g_pair_mode = mode;
-}
-static int g_dual_mode = 1;    // 1: single-CTA launches use the DUAL form (default), 0: never
+static int g_dual_mode = 1;    // 1: conv_tc_kernel launches use the DUAL form (default), 0: never
 void tc_debug_dual_mode(int mode) { g_dual_mode = mode; }
-static int g_pair_dual = 1;    // 1: CTA pairs use the DUAL form as well (default), 0: the plain three-instruction pair form
-void tc_debug_pair_dual(int on) { g_pair_dual = on; }
 // HALO form wherever legal (see tc_make_launch); env DDNM_HALO=0 / tc_debug_halo(0) keep every launch on one A load per k-block
 static int g_halo_enable = [] { const char* v = std::getenv("DDNM_HALO"); return v && *v ? std::atoi(v) : 1; }();
 void tc_debug_halo(int on) { g_halo_enable = on; }
-// ping-pong kernel for the single-CTA launches without the GN form (see tc_run); env DDNM_PINGPONG=0 / tc_debug_pingpong(0) keep
+// ping-pong kernel for the launches where CTAs walk several tiles (see tc_run); env DDNM_PINGPONG=0 / tc_debug_pingpong(0) keep
 // them on conv_tc_kernel
 static int g_pingpong_enable = [] { const char* v = std::getenv("DDNM_PINGPONG"); return v && *v ? std::atoi(v) : 1; }();
 void tc_debug_pingpong(int on) { g_pingpong_enable = on; }
@@ -1022,16 +890,9 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
     if (g_force_bn && Cout % g_force_bn == 0) L.BN = g_force_bn;   // tests / tuning experiments only
   }
   p.n_tiles = Cout / L.BN;
-  // CTA pairs (B tile multicast to two CTAs of a cluster) need an even number of M tiles and one weight matrix for all images.
-  // Not the default: on an H100 SXM at a 400 W limit the celeba forward (B = 16) took 80.5 ms with pairs on every layer of at least
-  // two waves of tiles and 74.6 ms without — the weight traffic they save is not what limits these layers.
-  {
-    const int m_tiles = p.tiles_x * p.tiles_y * p.tiles_n;
-    L.pair = !invariant && g_pair_mode == 1 && w_batches == 1 && m_tiles % 2 == 0;
-  }
   // batch-invariant launches run the three-instruction form, which conv_tc_kernel without DUAL and the ping-pong kernel share
   // element for element, so the kernel a launch picks (tc_run: tiles per CTA) cannot change a value
-  L.dual = !invariant && g_dual_mode != 0 && (!L.pair || g_pair_dual != 0);
+  L.dual = !invariant && g_dual_mode != 0;
   L.pingpong = g_pingpong_enable != 0;
   p.mode0 = mode0;
   p.cb0 = src0.C / BK;
@@ -1067,7 +928,7 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
   // halo maps are kept next to the plain ones: a launch that is later split along K (UNetEngine::emit_tc) runs without them.
   // Not with a 1x1 side input: its k-blocks have no taps to share, and as one A unit each they left the celeba conv2 + shortcut
   // launches at 128^2 / 256^2 up to 12 % slower than the per-tap form (whole forward: 60.1 ms with them in the HALO form, 58.2 without).
-  L.halo = g_halo_enable != 0 && !L.pair && (mode0 == TAPS_3X3 || mode0 == TAPS_UP2X2) && p.bw % 64 == 0 && p.bn == 1 && !src1;
+  L.halo = g_halo_enable != 0 && (mode0 == TAPS_3X3 || mode0 == TAPS_UP2X2) && p.bw % 64 == 0 && p.bn == 1 && !src1;
   if (L.halo) {
     const uint32_t hbox[4] = {(uint32_t)BK, (uint32_t)(p.bw + (mode0 == TAPS_UP2X2 ? 1 : 2)), (uint32_t)p.bh, 1u};
     L.hh = make_map_f16(src0.hi, 4, ad, hbox);
@@ -1083,24 +944,23 @@ TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1,
   }
   const int Ktot = (p.kb0 + p.kb1) * BK;
   const uint64_t bd[3] = {(uint64_t)Ktot, (uint64_t)Cout, (uint64_t)w_batches};
-  const uint32_t bbox[3] = {(uint32_t)BK, (uint32_t)(L.pair ? L.BN / 2 : L.BN), 1u};   // PAIR: each CTA loads half of the B tile
+  const uint32_t bbox[3] = {(uint32_t)BK, (uint32_t)L.BN, 1u};
   L.bh = make_map_f16(w_hi, 3, bd, bbox);
   L.bl = make_map_f16(w_lo, 3, bd, bbox);
   // ping-pong CTA pairs (one weight matrix; tc_run takes them when the launch runs on the ping-pong kernel unsplit).  Not for the
   // upsample phases: celeba B = 16 on an H100 SXM (700 W) ran the 128 -> 256 phases 8 % slower paired, the 256^2 / 128^2 3x3
   // launches 3-11 % faster.
-  L.pp_pair = g_pp_pair_enable != 0 && !L.pair && w_batches == 1 && mode0 != TAPS_UP2X2;
+  L.pp_pair = g_pp_pair_enable != 0 && w_batches == 1 && mode0 != TAPS_UP2X2;
   if (L.pp_pair) {
     const uint32_t hbox[3] = {(uint32_t)BK, (uint32_t)(L.BN / 2), 1u};
     L.bh2 = make_map_f16(w_hi, 3, bd, hbox);
     L.bl2 = make_map_f16(w_lo, 3, bd, hbox);
   }
   const int total = p.tiles_x * p.tiles_y * p.tiles_n * p.n_tiles;
-  L.grid = L.pair ? 2 * std::min(total / 2, num_sms / 2) : std::min(total, num_sms);
+  L.grid = std::min(total, num_sms);
   // contiguous tile ranges per CTA where the GroupNorm sums of the output would otherwise be flushed at every tile: one N tile
   // (so consecutive tiles of a range share their channels) and several tiles per CTA
-  const int units = L.pair ? total / 2 : total, workers = L.pair ? L.grid / 2 : L.grid;
-  p.deal = g_deal >= 0 ? g_deal : (out.st != nullptr && p.n_tiles == 1 && units >= 2 * workers ? 1 : 0);
+  p.deal = g_deal >= 0 ? g_deal : (out.st != nullptr && p.n_tiles == 1 && total >= 2 * L.grid ? 1 : 0);
   if (p.n_tiles != 1) p.deal = 0;
   L.flops = 2.0 * (double)out.pixels() * Cout * Ktot;
   return L;
@@ -1170,15 +1030,14 @@ TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, 
   return L;
 }
 
-template <int BN, bool PAIR, bool DUAL, bool GN = false, bool HALO = false, bool NTAIL = false>
+template <int BN, bool DUAL, bool HALO = false, bool NTAIL = false>
 static void launch_bn(const TcLaunch& L, cudaStream_t stream) {
   using Cfg = TcCfg<BN, DUAL, HALO>;
   static bool attr_set[64] = {};
   if (first_use_on_device(attr_set))
-    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_kernel<BN, PAIR, DUAL, GN, HALO, NTAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    Cfg::SMEM_BYTES));
-  launch_pdl(conv_tc_kernel<BN, PAIR, DUAL, GN, HALO, NTAIL>, dim3(L.grid), dim3(kTcThreads), (size_t)Cfg::SMEM_BYTES, stream, PAIR ? 2 : 1,
-             HALO ? L.hh : L.a0h, HALO ? L.hl : L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.p, L.g);
+    CUDA_CHECK(cudaFuncSetAttribute(conv_tc_kernel<BN, DUAL, HALO, NTAIL>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+  launch_pdl(conv_tc_kernel<BN, DUAL, HALO, NTAIL>, dim3(L.grid), dim3(kTcThreads), (size_t)Cfg::SMEM_BYTES, stream, 1,
+             HALO ? L.hh : L.a0h, HALO ? L.hl : L.a0l, L.a1h, L.a1l, L.bh, L.bl, L.p);
   CUDA_CHECK(cudaGetLastError());
 }
 
@@ -1186,20 +1045,16 @@ template <int BN>
 static void launch_forms(const TcLaunch& L, cudaStream_t stream) {
   if (L.ntail) {   // batched GEMMs with a partial N tile: N % 64 != 0, so BN = 64
     if constexpr (BN == 64) {
-      if (L.dual) launch_bn<BN, false, true, false, false, true>(L, stream);
-      else launch_bn<BN, false, false, false, false, true>(L, stream);
+      if (L.dual) launch_bn<BN, true, false, true>(L, stream);
+      else launch_bn<BN, false, false, true>(L, stream);
       return;
     }
     throw Error("partial N tiles need BN = 64");
   }
-  if (L.halo && L.dual) launch_bn<BN, false, true, false, true>(L, stream);
-  else if (L.halo) launch_bn<BN, false, false, false, true>(L, stream);
-  else if (L.gn && L.dual) launch_bn<BN, false, true, true>(L, stream);
-  else if (L.gn) launch_bn<BN, false, false, true>(L, stream);
-  else if (L.pair && L.dual) launch_bn<BN, true, true>(L, stream);
-  else if (L.pair) launch_bn<BN, true, false>(L, stream);
-  else if (L.dual) launch_bn<BN, false, true>(L, stream);
-  else launch_bn<BN, false, false>(L, stream);
+  if (L.halo && L.dual) launch_bn<BN, true, true>(L, stream);
+  else if (L.halo) launch_bn<BN, false, true>(L, stream);
+  else if (L.dual) launch_bn<BN, true>(L, stream);
+  else launch_bn<BN, false>(L, stream);
 }
 
 template <int BN, int TERMS, bool HALO, bool NTAIL = false, bool PAIR = false>
@@ -1270,63 +1125,12 @@ static void launch_pingpong_forms(const TcLaunch& L, cudaStream_t stream) {
   else launch_pingpong_terms<BN, false>(L, stream);
 }
 
-// ---- GN form: fused GroupNorm + SiLU + split + 3x3 convolution ----
-// Default OFF (env DDNM_GN_FUSED=1 / ddnm_tc_debug_gn_fused): per launch it saves the normalised planes' HBM round trip, but every
-// consumer warpgroup then waits for its own row loads before each k-block's MMAs.
-static int g_gn_enable = [] { const char* v = std::getenv("DDNM_GN_FUSED"); return v && *v ? std::atoi(v) : 0; }();
-void tc_debug_gn_fused(int on) { g_gn_enable = on; }
-
-static bool gn_shape_ok(const View& x, const View* side, int Cout, const View& out) {
-  if (out.W % 128 != 0 || x.C % BK != 0 || x.C > kGnMaxC || Cout % 64 != 0) return false;
-  if (x.H != out.H || x.W != out.W || x.N != out.N) return false;
-  if (x.ld % 4 != 0 || ((uintptr_t)x.p & 15) != 0) return false;
-  if (side && (side->C % BK != 0 || side->ld % 4 != 0 || ((uintptr_t)side->p & 15) != 0 || side->H != out.H || side->W != out.W ||
-               side->N != out.N))
-    return false;
-  return true;
-}
-
-bool tc_gn_eligible(const View& x, const View* side, int Cout, const View& out) { return g_gn_enable != 0 && gn_shape_ok(x, side, Cout, out); }
-
-TcLaunch tc_make_gn_launch(const View& x, const GnAffine& gn, const View* side, const __half* w_hi, const __half* w_lo, int Cout,
-                           const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int num_sms) {
-  DDNM_CHECK(gn_shape_ok(x, side, Cout, out), "fused GroupNorm convolution: unsupported shape");
-  DDNM_CHECK(g_terms == 3, "the fused GroupNorm convolution implements the fp32-grade (3-term) arithmetic only");
-  // the tiling, B operand and epilogue of a plain 3x3 launch over a placeholder A split of x's shape (its tensor maps are unused)
-  SplitView a;
-  a.hi = const_cast<__half*>(w_hi);
-  a.lo = const_cast<__half*>(w_lo);
-  a.N = x.N; a.H = x.H; a.W = x.W; a.C = x.C;
-  SplitView s1;
-  if (side) {
-    s1 = a;
-    s1.C = side->C;
-  }
-  const int gp = g_pair_mode;
-  g_pair_mode = 0;
-  TcLaunch L = tc_make_launch(a, TAPS_3X3, side ? &s1 : nullptr, w_hi, w_lo, 1, Cout, out, chanadd, ca_ld, residual, ldr, 1.0f, num_sms, 0);
-  g_pair_mode = gp;
-  L.gn = true;
-  L.halo = false;
-  L.dual = L.dual && L.BN == 64;   // GN + DUAL at BN = 128 exceeds the 168 registers per thread of three warpgroups (spills)
-  TcGnArgs& g = L.g;
-  g.x = x.p; g.x_ld = x.ld; g.C = x.C;
-  g.xs = side ? side->p : nullptr; g.xs_ld = side ? side->ld : 0;
-  g.norm = gn.gamma != nullptr ? 1 : 0;
-  if (g.norm) DDNM_CHECK(x.st != nullptr && x.C % gn.groups == 0, "normalisation needs the tensor's per-channel sums (View::st)");
-  g.st = x.st; g.st_ld = x.st_ld;
-  g.gamma = gn.gamma; g.beta = gn.beta; g.eps = gn.eps; g.groups = gn.groups; g.ss = gn.ss; g.ss_ld = gn.ss_ld; g.silu = gn.silu ? 1 : 0;
-  return L;
-}
-
 void tc_run(const TcLaunch& L, cudaStream_t stream) {
-  DDNM_CHECK(!L.pair || L.p.split_k == 1, "CTA pairs do not split K");
-  DDNM_CHECK(!L.halo || (L.p.split_k == 1 && !L.pair && !L.gn && L.p.kb1 == 0),
-             "the HALO form runs unsplit single-CTA launches with TMA-loaded A and no 1x1 side input");
+  DDNM_CHECK(!L.halo || (L.p.split_k == 1 && L.p.kb1 == 0), "the HALO form runs unsplit launches without a 1x1 side input");
   // ping-pong needs two tiles per CTA to overlap one tile's epilogue with the next one's MMAs; a CTA with one tile (the split-K
   // launches, the 16x16 level) runs faster on two warpgroups sharing it
   const int units = L.p.tiles_x * L.p.tiles_y * L.p.tiles_n * L.p.n_tiles * L.p.split_k;
-  if (L.pingpong && !L.pair && !L.gn && units > L.grid) {
+  if (L.pingpong && units > L.grid) {
     switch (L.BN) {
       case 128: launch_pingpong_forms<128>(L, stream); return;
       case 64: launch_pingpong_forms<64>(L, stream); return;

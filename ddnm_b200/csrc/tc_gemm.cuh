@@ -43,37 +43,17 @@ struct TcParams {
                                //    carried into the CTA's next tile, so their grouping depends only on the tile's place in its image
 };
 
-// GN form (fused GroupNorm + SiLU + split + 3x3 convolution, see conv_tc_kernel): the A operand is produced from fp32 rows
-struct TcGnArgs {
-  const float* x = nullptr;       // fp32 NHWC source of the 3x3 taps, row pitch x_ld, C channels
-  int x_ld = 0, C = 0;
-  const float* xs = nullptr;      // optional fp32 NHWC raw input of the 1x1 shortcut (extra K blocks), row pitch xs_ld
-  int xs_ld = 0;
-  const StatAcc* st = nullptr;    // per-(image, channel) sums of x (View::st)
-  int st_ld = 0;
-  const float* gamma = nullptr;
-  const float* beta = nullptr;
-  float eps = 0.f;
-  int groups = 32;
-  const float* ss = nullptr;      // optional per-(image, channel) [scale(C) | shift(C)] rows (use_scale_shift_norm)
-  int ss_ld = 0;
-  int silu = 0, norm = 0;
-};
-
 struct TcLaunch {
-  CUtensorMap a0h, a0l, a1h, a1l, bh, bl;   // PAIR: bh / bl have a BN/2-row box (each CTA of the pair loads half of the B tile)
+  CUtensorMap a0h, a0l, a1h, a1l, bh, bl;
   CUtensorMap hh, hl;          // HALO: source 0 with a halo-row box {64, bw + 2 (up2: bw + 1), bh, 1}
   TcParams p;
   int BN = 128;
-  bool pair = false;           // CTA-pair kernel (cluster of 2, B tile multicast to both CTAs)
   bool dual = false;           // A_hi x [B_hi; B_lo] as one m64 x 2BN instruction, two partial accumulators
-  bool gn = false;             // GN form: A produced in the kernel from g
   bool halo = false;           // HALO form: one A load per (dy, channel slice) feeds the dx taps; needs split_k == 1
   bool pingpong = false;       // ping-pong kernel where the launch allows it (see tc_run); DUAL does not apply there
   bool pp_pair = false;        // the ping-pong launch may run on CTA pairs (see tc_make_launch); bh2 / bl2 have the BN/2-row box
   CUtensorMap bh2, bl2;
   bool ntail = false;          // batched GEMM whose N is not a multiple of BN: the last N tile is partial (never a convolution)
-  TcGnArgs g;
   int grid = 0;
   double flops = 0;            // algorithmic flops (2*M*N*K, counted once)
 };
@@ -81,7 +61,7 @@ struct TcLaunch {
 // Build the launch record.  src0/src1: fp16 split activations; w_hi/w_lo: [batch][Cout][Ktot] fp16 K-major with
 // Ktot = taps*C0 + C1 (k index = tap*C0 + ci, then source-1 channels).
 // invariant: batch-invariant launch — an output element's arithmetic depends only on its image and the layer's shape, not on
-// the batch, the image's place in it or num_sms (no DUAL form, no CTA pairs of conv_tc_kernel, GroupNorm partials flushed per tile)
+// the batch, the image's place in it or num_sms (no DUAL form, GroupNorm partials flushed per tile)
 TcLaunch tc_make_launch(const SplitView& src0, int mode0, const SplitView* src1, const __half* w_hi, const __half* w_lo,
                         int w_batches, int Cout, const View& out, const float* chanadd, int ca_ld, const float* residual,
                         int ldr, float alpha, int num_sms, int res_mode = 0, bool invariant = false);
@@ -104,29 +84,10 @@ struct GemmOperand {
 TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, int N, int K, int heads, int images, float* out,
                              long long out_sn, long long out_sy, long long out_sx, float alpha, int num_sms, bool invariant = false);
 
-// ---- fused GroupNorm + SiLU + split + 3x3 convolution (the GN form of conv_tc_kernel) ----
-struct GnAffine {
-  const float* gamma = nullptr;   // nullptr: no normalisation (raw split)
-  const float* beta = nullptr;
-  float eps = 1e-6f;
-  int groups = 32;
-  bool silu = true;
-  const float* ss = nullptr;      // optional per-(image, channel) [scale(C) | shift(C)] rows (use_scale_shift_norm, unet.py:250-252)
-  int ss_ld = 0;
-};
-// x: fp32 activation with its GroupNorm sums; side: raw fp32 input of a 1x1 shortcut riding as extra K blocks (may be null);
-// w_hi/w_lo as for tc_make_launch with Ktot = 9*x.C + side.C.
-bool tc_gn_eligible(const View& x, const View* side, int Cout, const View& out);
-TcLaunch tc_make_gn_launch(const View& x, const GnAffine& gn, const View* side, const __half* w_hi, const __half* w_lo, int Cout,
-                           const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int num_sms);
-void tc_debug_gn_fused(int on);      // 1: eligible layers of engines built afterwards use the GN form; 0 (default): gn_apply + conv_tc
-
 // debug knobs (tests only): apply to the launches built afterwards
 void tc_debug_force_bn(int bn);      // 0 (default): heuristic, 64 / 128: force the N tile where Cout (GEMM: N) allows it
 void tc_debug_deal(int mode);        // -1 (default): contiguous tile ranges where they pay (one N tile + GroupNorm sums), 0 / 1: force
-void tc_debug_pair_mode(int mode);   // -1 (default) / 0: no CTA pairs, 1: CTA pairs wherever legal
-void tc_debug_dual_mode(int mode);   // 1 (default): DUAL form for single-CTA launches, 0: never
-void tc_debug_pair_dual(int on);     // 1 (default): CTA pairs use the DUAL form too, 0: the plain pair form
+void tc_debug_dual_mode(int mode);   // 1 (default): DUAL form for conv_tc_kernel launches, 0: never
 void tc_debug_halo(int on);          // 1 (default, env DDNM_HALO): HALO form wherever legal, 0: never
 void tc_debug_pingpong(int on);      // 1 (default, env DDNM_PINGPONG): ping-pong kernel wherever it applies, 0: never
 void tc_debug_pp_pair(int on);       // 1 (default, env DDNM_PP_PAIR): ping-pong launches on CTA pairs where legal, 0: single CTAs

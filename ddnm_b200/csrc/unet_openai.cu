@@ -30,22 +30,6 @@ void UNetOpenAI::emit_resblock(const std::string& p, const View& x, const View& 
   View h;
   h.p = hbuf_; h.N = B_; h.H = out.H; h.W = out.W; h.C = Cout; h.ld = Cout;
   h.st = new_stats(Cout); h.st_ld = Cout;   // conv1's epilogue accumulates the sums out_layers.0 needs
-  if (kind == RES_PLAIN && fused_ok(x, nullptr, Cout, h) && fused_ok(h, has_skip_conv ? &x : nullptr, Cout, out)) {
-    // wide maps: GroupNorm (+ scale-shift) + SiLU + fp16 split inside the convolution kernel (conv_tc_kernel's GN form)
-    TcWeights w1 = prep_weights(p + ".in_layers.2.weight", Cout, Cin, 9, "", 0);
-    emit_tcgn(p + ".conv1", x, p + ".in_layers.0", nullptr, 0, nullptr, w1, Cout, h, P(p + ".in_layers.2.bias", Cout), 0, nullptr, 0);
-    if (has_skip_conv) {
-      TcWeights w2 = prep_weights(p + ".out_layers.3.weight", Cout, Cout, 9, p + ".skip_connection.weight", Cin);
-      emit_tcgn(p + ".conv2+skip", h, p + ".out_layers.0", ss_all_ + ss_off_.at(p), ss_total_, &x, w2, Cout, out,
-                bias_sum(p + ".out_layers.3.bias", p + ".skip_connection.bias", Cout), 0, nullptr, 0);
-    } else {
-      DDNM_CHECK(Cin == Cout, "identity skip needs equal channels");
-      TcWeights w2 = prep_weights(p + ".out_layers.3.weight", Cout, Cout, 9, "", 0);
-      emit_tcgn(p + ".conv2", h, p + ".out_layers.0", ss_all_ + ss_off_.at(p), ss_total_, nullptr, w2, Cout, out,
-                P(p + ".out_layers.3.bias", Cout), 0, x.p, x.ld);
-    }
-    return;
-  }
   emit_gn_split(p + ".in", x, p + ".in_layers.0", true, mode1, A, nullptr, 0, has_skip_conv ? &Bs : nullptr);
   if (kind == RES_UP) {
     // in_conv(nearest_up(SiLU(GN(x)))) as four 2x2 parity-phase convolutions on the low-res activation

@@ -18,21 +18,6 @@ void UNetSimple::emit_resblock(const std::string& p, const View& x, const View& 
   View h;
   h.p = hbuf_; h.N = B_; h.H = x.H; h.W = x.W; h.C = Cout; h.ld = Cout;
   h.st = new_stats(Cout); h.st_ld = Cout;   // conv1's epilogue accumulates the sums norm2 needs
-  if (fused_ok(x, nullptr, Cout, h) && fused_ok(h, Cin != Cout ? &x : nullptr, Cout, out)) {
-    // wide maps (rows >= 128 pixels): GroupNorm + SiLU + fp16 split happen inside the convolution kernels, the planes never
-    // reach HBM; the 1x1 shortcut's raw input is split by conv2's transform warps as well
-    TcWeights w1 = prep_weights(p + ".conv1.weight", Cout, Cin, 9, "", 0);
-    emit_tcgn(p + ".conv1", x, p + ".norm1", nullptr, 0, nullptr, w1, Cout, h, ca_all_ + ca_off_.at(p), ca_total_, nullptr, 0);
-    if (Cin != Cout) {
-      TcWeights w2 = prep_weights(p + ".conv2.weight", Cout, Cout, 9, p + ".nin_shortcut.weight", Cin);
-      emit_tcgn(p + ".conv2+nin", h, p + ".norm2", nullptr, 0, &x, w2, Cout, out,
-                bias_sum(p + ".conv2.bias", p + ".nin_shortcut.bias", Cout), 0, nullptr, 0);
-    } else {
-      TcWeights w2 = prep_weights(p + ".conv2.weight", Cout, Cout, 9, "", 0);
-      emit_tcgn(p + ".conv2", h, p + ".norm2", nullptr, 0, nullptr, w2, Cout, out, P(p + ".conv2.bias", Cout), 0, x.p, x.ld);
-    }
-    return;
-  }
   // blocks with a 1x1 shortcut also need the raw split of x: produced by the same pass that normalises it
   emit_gn_split(p + ".norm1", x, p + ".norm1", true, SPLIT_SAME, A, nullptr, 0, Cin != Cout ? &Bs : nullptr);
   TcWeights w1 = prep_weights(p + ".conv1.weight", Cout, Cin, 9, "", 0);

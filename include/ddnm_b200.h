@@ -320,35 +320,20 @@ int ddnm_conv_tc_bench(int N, int H, int W, int Cin, int Cout, int mode, int ite
 int ddnm_gnconv_chunk_bench(int N, int chunk, int H, int W, int Cin, int Cout, int iters, float* ms_per_pass);
 int ddnm_groupnorm(const float* x, int N, int H, int W, int C, int groups, const float* gamma, const float* beta, float eps,
                    int silu, float* out, void* stream);
-/* out = conv3x3(silu?(groupnorm(x))) [+ conv1x1(side_x)] + bias [+ residual] with the GroupNorm / SiLU / fp16 split applied INSIDE the
- * convolution kernel (models.py:115-134 conv1 / conv2 + nin_shortcut), rows of >= 128 pixels.  gamma == NULL: no normalisation.
- * iters > 0 additionally times `iters` launches into *ms_per_iter. */
-int ddnm_conv_gn_tc(const float* x, int N, int H, int W, int Cin, int groups, const float* gamma, const float* beta, float eps, int silu,
-                    const float* w, const float* bias, int Cout, const float* side_x, int CinSide, const float* side_w,
-                    const float* residual, float* out, int iters, float* ms_per_iter, void* stream);
-/* 1: eligible layers (3x3, rows >= 128 pixels) of engines built afterwards run the fused GroupNorm convolution; 0 (default, also env
- * DDNM_GN_FUSED): gn_apply_kernel + conv_tc_kernel */
-int ddnm_tc_debug_gn_fused(int on);
 /* tuning experiments: force the N-tile width (64 or 128) of conv and attention-GEMM launches built afterwards where the output
  * width allows it (0 = heuristic) */
 int ddnm_tc_debug_force_bn(int bn);
 /* tile -> CTA map of conv launches built afterwards: -1 (default) contiguous tile ranges per CTA on layers with one N tile that
  * produce GroupNorm sums, 0 round-robin everywhere, 1 contiguous wherever legal */
 int ddnm_tc_debug_deal(int mode);
-/* CTA pairs (cluster of 2 sharing the weight tile through TMA multicast) for conv launches built afterwards: -1 (default) and 0
- * never (slower than single CTAs on the H100 networks), 1 wherever legal */
-int ddnm_tc_debug_pair_mode(int mode);
 /* 1 (default): single-CTA launches issue hi*hi and hi*lo as one m64 x 2BN instruction (two partial accumulators); 0: never */
 int ddnm_tc_debug_dual_mode(int mode);
-/* 1 (default): CTA pairs use that DUAL form as well; 0: the plain three-instruction pair form */
-int ddnm_tc_debug_pair_dual(int on);
 /* 1 (default, also env DDNM_HALO): 3x3 stride-1 and upsample-phase conv launches built afterwards on maps >= 64 px wide and without
  * a 1x1 side input load each
  * (dy, 64-channel slice) of the activation once as halo rows for all column taps; 0: one A load per tap */
 int ddnm_tc_debug_halo(int on);
-/* 1 (default, also env DDNM_PINGPONG): single-CTA launches without the fused GroupNorm form, built afterwards, run on the ping-pong
- * kernel (two consumer warpgroups that each own a whole tile and take turns on the tensor cores) where a CTA gets at least two tiles;
- * 0: never */
+/* 1 (default, also env DDNM_PINGPONG): conv and attention-GEMM launches built afterwards run on the ping-pong kernel (two consumer
+ * warpgroups that each own a whole tile and take turns on the tensor cores) where a CTA gets at least two tiles; 0: never */
 int ddnm_tc_debug_pingpong(int on);
 /* 1 (default, also env DDNM_PP_PAIR): ping-pong launches (not the upsample phases), built afterwards, run on clusters of two CTAs that each
  * load half of every weight k-block and multicast it to both (bit-identical output); 0: single CTAs */

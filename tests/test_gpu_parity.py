@@ -53,7 +53,9 @@ def _conv_ref(x, w, b, mode=0, up2=False, side=None, side_w=None, res=None):
 
 
 @pytest.mark.parametrize("shape", [(1, 16, 16, 64, 64, 0), (2, 32, 32, 128, 128, 0), (1, 64, 64, 128, 256, 0), (3, 8, 8, 128, 64, 0),
-                                   (1, 128, 128, 192, 128, 0), (1, 16, 16, 512, 1536, 1), (2, 32, 32, 128, 128, 2), (3, 16, 16, 64, 64, 2)],
+                                   (1, 128, 128, 192, 128, 0), (1, 16, 16, 512, 1536, 1), (2, 32, 32, 128, 128, 2), (3, 16, 16, 64, 64, 2),
+                                   (2, 256, 256, 64, 128, 0), (4, 128, 128, 128, 256, 0), (4, 128, 128, 128, 128, 0), (4, 128, 128, 64, 128, 1),
+                                   (8, 128, 128, 64, 128, 2), (2, 128, 128, 64, 384, 0)],
                          ids=str)
 def test_tc_conv_vs_fp64(lib, shape):
     # tolerance: fp32 accumulation over K <= 4608 terms on the tensor core (truncating adds) gives ~3e-6 relative to the
@@ -85,37 +87,27 @@ def test_tc_conv_fusions(lib):
     lib.check(L.ddnm_conv_direct(lib.ptr(x.permute(0, 2, 3, 1).contiguous()), N, H, W, Cin, lib.ptr(w), lib.ptr(b), Cout, 0, 0, lib.ptr(out), None))
     torch.cuda.synchronize()
     assert_close(_conv_tc(lib, x, w, b), out.permute(0, 3, 1, 2), 1e-4, 5e-5, "tc vs direct")
-
-
-@pytest.mark.parametrize("shape", [(2, 256, 256, 64, 128, 0), (4, 128, 128, 128, 256, 0), (4, 128, 128, 64, 128, 1), (8, 128, 128, 64, 128, 2),
-                                   (2, 128, 128, 64, 384, 0)], ids=str)
-def test_tc_conv_cta_pair_vs_fp64_and_single_cta(lib, shape):
-    """CTA-pair kernel (cluster of two CTAs on M-adjacent tiles, each loading half of the weight tile and multicasting it to both):
-    it must agree with the fp64 reference AND with the single-CTA kernel on the same inputs."""
-    N, H, W, Cin, Cout, mode = shape
-    torch.manual_seed(5)
-    k = 1 if mode == 1 else 3
+    # the same fusions on maps where CTAs walk several tiles (ping-pong, CTA pairs, HALO)
+    torch.manual_seed(6)
+    N, H, W, Cin, Cout = 8, 64, 64, 64, 128
     x = torch.randn(N, Cin, H, W, device=dev)
-    w = torch.randn(Cout, Cin, k, k, device=dev) / (k * k * Cin) ** 0.5
+    w = torch.randn(Cout, Cin, 3, 3, device=dev) / (9 * Cin) ** 0.5
     b = torch.randn(Cout, device=dev)
-    L = lib.lib()
-    try:
-        lib.check(L.ddnm_tc_debug_pair_mode(0))
-        single = _conv_tc(lib, x, w, b, mode=mode).clone()
-        lib.check(L.ddnm_tc_debug_pair_mode(1))
-        lib.check(L.ddnm_tc_debug_pair_dual(0))          # the plain pair form; PAIR + DUAL has its own test
-        pair = _conv_tc(lib, x, w, b, mode=mode)
-    finally:
-        L.ddnm_tc_debug_pair_mode(-1)
-        L.ddnm_tc_debug_pair_dual(1)
-    torch.cuda.synchronize()
-    # same products; the two forms may differ by fp32 re-association (DUAL vs three-instruction accumulation); both sit inside
-    # the fp64 tolerance below
-    assert_close(pair, single, 3e-5, 2e-5, f"pair vs single-CTA {shape}")
-    assert_close(pair, _conv_ref(x, w, b, mode=mode), rtol=1e-4, atol=5e-5, what=f"pair conv {shape}")
+    assert_close(_conv_tc(lib, x, w, b, up2=True), _conv_ref(x, w, b, up2=True), 1e-4, 5e-5, "upsample conv (four parity phases), 8x64x64")
+    N, H, W = 4, 128, 128
+    x = torch.randn(N, Cin, H, W, device=dev)
+    res = torch.randn(N, Cout, H, W, device=dev)
+    side = torch.randn(N, 128, H, W, device=dev)
+    sw = torch.randn(Cout, 128, 1, 1, device=dev) / 128 ** 0.5
+    assert_close(_conv_tc(lib, x, w, b, res=res), _conv_ref(x, w, b, res=res), 1e-4, 5e-5, "residual epilogue, 4x128x128")
+    assert_close(_conv_tc(lib, x, w, b, side=side, side_w=sw), _conv_ref(x, w, b, side=side, side_w=sw), 1e-4, 5e-5,
+                 "1x1 side input, 4x128x128")
 
 
-@pytest.mark.parametrize("shape", [(2, 32, 32, 128, 128, 0), (1, 64, 64, 128, 256, 0), (3, 8, 8, 128, 64, 0), (2, 64, 64, 192, 128, 1)], ids=str)
+# at most one tile per SM, so both forms run on conv_tc_kernel: BN = 64 and 128, with and without HALO, 1x1 and stride 2
+@pytest.mark.parametrize("shape", [(2, 32, 32, 128, 128, 0), (1, 64, 64, 128, 256, 0), (3, 8, 8, 128, 64, 0), (2, 64, 64, 192, 128, 1),
+                                   (1, 128, 128, 128, 128, 0), (16, 32, 32, 128, 128, 0), (2, 16, 16, 256, 512, 0), (1, 64, 64, 128, 128, 2)],
+                         ids=str)
 def test_tc_conv_dual_accumulator_vs_three_instruction_form(lib, shape):
     """DUAL kernel (hi*hi and hi*lo issued as one m64 x 2BN wgmma over the adjacent B_hi / B_lo planes, partial sums added in the
     epilogue) against the plain three-instruction form: the same products, two fp32 additions re-associated."""
@@ -128,120 +120,14 @@ def test_tc_conv_dual_accumulator_vs_three_instruction_form(lib, shape):
     L = lib.lib()
     try:
         lib.check(L.ddnm_tc_debug_dual_mode(0))
-        lib.check(L.ddnm_tc_debug_pair_mode(0))
         plain = _conv_tc(lib, x, w, b, mode=mode).clone()
         lib.check(L.ddnm_tc_debug_dual_mode(1))
         dual = _conv_tc(lib, x, w, b, mode=mode)
     finally:
         L.ddnm_tc_debug_dual_mode(1)
-        L.ddnm_tc_debug_pair_mode(-1)
     torch.cuda.synchronize()
     assert_close(dual, plain, 2e-5, 1e-5, f"dual vs plain {shape}")
     assert_close(dual, _conv_ref(x, w, b, mode=mode), rtol=1e-4, atol=5e-5, what=f"dual conv {shape}")
-
-
-@pytest.mark.parametrize("shape", [(2, 256, 256, 64, 128, 0), (4, 128, 128, 128, 128, 0), (4, 128, 128, 64, 128, 1), (8, 128, 128, 64, 128, 2),
-                                   (2, 128, 128, 64, 384, 0)], ids=str)
-def test_tc_conv_pair_dual_form(lib, shape):
-    """PAIR + DUAL at BN = 128: the CTA pair's multicast weight halves feed the DUAL form's m64 x 256 A_hi x [B_hi; B_lo]
-    instruction, plus A_lo x B_hi into the first half of the accumulator."""
-    N, H, W, Cin, Cout, mode = shape
-    torch.manual_seed(8)
-    k = 1 if mode == 1 else 3
-    x = torch.randn(N, Cin, H, W, device=dev)
-    w = torch.randn(Cout, Cin, k, k, device=dev) / (k * k * Cin) ** 0.5
-    b = torch.randn(Cout, device=dev)
-    L = lib.lib()
-    try:
-        lib.check(L.ddnm_tc_debug_pair_mode(0))
-        single = _conv_tc(lib, x, w, b, mode=mode).clone()
-        lib.check(L.ddnm_tc_debug_pair_mode(1))
-        lib.check(L.ddnm_tc_debug_pair_dual(1))
-        lib.check(L.ddnm_tc_debug_force_bn(128))
-        pd = _conv_tc(lib, x, w, b, mode=mode)
-    finally:
-        L.ddnm_tc_debug_pair_mode(-1)
-        L.ddnm_tc_debug_pair_dual(1)
-        L.ddnm_tc_debug_force_bn(0)
-    torch.cuda.synchronize()
-    assert_close(pd, single, 3e-5, 2e-5, f"pair+dual vs single-CTA {shape}")
-    assert_close(pd, _conv_ref(x, w, b, mode=mode), rtol=1e-4, atol=5e-5, what=f"pair+dual conv {shape}")
-
-
-def test_tc_conv_cta_pair_fusions(lib):
-    torch.manual_seed(6)
-    L = lib.lib()
-    lib.check(L.ddnm_tc_debug_pair_mode(1))
-    try:
-        _pair_fusions(lib)
-    finally:
-        L.ddnm_tc_debug_pair_mode(-1)
-
-
-def _pair_fusions(lib):
-    N, H, W, Cin, Cout = 8, 64, 64, 64, 128
-    x = torch.randn(N, Cin, H, W, device=dev)
-    w = torch.randn(Cout, Cin, 3, 3, device=dev) / (9 * Cin) ** 0.5
-    b = torch.randn(Cout, device=dev)
-    assert_close(_conv_tc(lib, x, w, b, up2=True), _conv_ref(x, w, b, up2=True), 1e-4, 5e-5, "pair: upsample conv (four parity phases)")
-    N, H, W = 4, 128, 128
-    x = torch.randn(N, Cin, H, W, device=dev)
-    res = torch.randn(N, Cout, H, W, device=dev)
-    side = torch.randn(N, 128, H, W, device=dev)
-    sw = torch.randn(Cout, 128, 1, 1, device=dev) / 128 ** 0.5
-    assert_close(_conv_tc(lib, x, w, b, res=res), _conv_ref(x, w, b, res=res), 1e-4, 5e-5, "pair: residual epilogue")
-    assert_close(_conv_tc(lib, x, w, b, side=side, side_w=sw), _conv_ref(x, w, b, side=side, side_w=sw), 1e-4, 5e-5, "pair: 1x1 side input")
-
-
-@pytest.mark.parametrize("shape", [(2, 128, 128, 128, 128, 0, False), (1, 256, 256, 64, 128, 0, True), (2, 128, 128, 128, 256, 0, False),
-                                   (2, 128, 128, 64, 128, 192, False), (1, 256, 256, 128, 256, 64, False), (4, 128, 128, 64, 128, 0, True)], ids=str)
-def test_fused_groupnorm_conv_vs_fp64(lib, shape):
-    """GN form of conv_tc_kernel: GroupNorm + SiLU + fp16 split applied INSIDE the wgmma convolution (each consumer warpgroup writes
-    its swizzled A rows from the fp32 input), with the 1x1 side input (nin_shortcut) and the residual epilogue — against an fp64
-    group_norm -> silu -> conv2d."""
-    N, H, W, Cin, Cout, side_c, res = shape
-    L = lib.lib()
-    torch.manual_seed(11)
-    x = torch.randn(N, Cin, H, W, device=dev) * 1.5 + 0.3
-    w = torch.randn(Cout, Cin, 3, 3, device=dev) / (9 * Cin) ** 0.5
-    b = torch.randn(Cout, device=dev)
-    g, be = torch.randn(Cin, device=dev), torch.randn(Cin, device=dev)
-    side = torch.randn(N, side_c, H, W, device=dev) if side_c else None
-    sw = (torch.randn(Cout, side_c, 1, 1, device=dev) / side_c ** 0.5).contiguous() if side_c else None
-    r = torch.randn(N, Cout, H, W, device=dev) if res else None
-    nhwc = lambda t: None if t is None else t.permute(0, 2, 3, 1).contiguous()   # noqa: E731
-    out = torch.empty(N, H, W, Cout, device=dev)
-    xs, ss, rs = nhwc(x), nhwc(side), nhwc(r)
-    lib.check(L.ddnm_conv_gn_tc(lib.ptr(xs), N, H, W, Cin, 32, lib.ptr(g), lib.ptr(be), 1e-6, 1, lib.ptr(w), lib.ptr(b), Cout, lib.ptr(ss), side_c,
-                                lib.ptr(sw), lib.ptr(rs), lib.ptr(out), 0, None, None))
-    torch.cuda.synchronize()
-    h = F.group_norm(x.double().cpu(), 32, g.double().cpu(), be.double().cpu(), 1e-6)
-    ref = F.conv2d(h * torch.sigmoid(h), w.double().cpu(), b.double().cpu(), padding=1)
-    if side is not None:
-        ref = ref + F.conv2d(side.double().cpu(), sw.double().cpu())
-    if r is not None:
-        ref = ref + r.double().cpu()
-    assert_close(out.permute(0, 3, 1, 2), ref, 1e-4, 1e-4, f"fused GroupNorm conv {shape}")
-
-
-def test_fused_and_unfused_engines_agree():
-    """The celeba network with the wide layers on the fused kernel vs the same network forced onto gn_apply + conv_tc."""
-    from ddnm_b200 import _lib as LL
-    cfg = U.SimpleUNetConfig.celeba_hq()
-    torch.manual_seed(23)
-    x = torch.randn(2, 3, 256, 256, device=dev)
-    t = torch.tensor([650.0, 12.0], device=dev)
-    LL.check(LL.lib().ddnm_tc_debug_gn_fused(1))
-    try:
-        fused = _engine_model(cfg)
-        a = fused(x, t)
-        LL.check(LL.lib().ddnm_tc_debug_gn_fused(0))
-        plain = _engine_model(cfg)
-        b = plain(x, t)
-    finally:
-        LL.lib().ddnm_tc_debug_gn_fused(0)
-    assert fused.info(2)["launches"] < plain.info(2)["launches"], "the fused engine must have fewer launches"
-    assert_close(a, b, 1e-4, 2e-5, "fused vs unfused celeba forward")
 
 
 def test_groupnorm_silu(lib):
