@@ -490,55 +490,6 @@ void UNetEncoder::emit_gn_backward(const std::string& name, const float* g, cons
   });
 }
 
-// ResBlock._forward (unet.py:236-256) with its activations kept for the backward pass
-void UNetEncoder::emit_resblock(const std::string& p, const View& x, const View& out, bool down, Layer& rec) {
-  const int Cin = x.C, Cout = out.C;
-  if (down) DDNM_CHECK(Cin == Cout, "down ResBlocks keep the channel count");
-  SplitView A{splitA_hi_, splitA_lo_}, Bs{splitB_hi_, splitB_lo_};
-  const bool skip = has_param(p + ".skip_connection.weight");
-  View h = new_view(out.H, out.W, Cout);
-  emit_gn_split(p + ".in", x, p + ".in_layers.0", true, down ? SPLIT_AVG2 : SPLIT_SAME, A, nullptr, 0, skip ? &Bs : nullptr);
-  TcWeights w1 = prep_weights(p + ".in_layers.2.weight", Cout, Cin, 9, "", 0);
-  emit_tc(p + ".conv1", A, TAPS_3X3, nullptr, w1, Cout, h, P(p + ".in_layers.2.bias", Cout), 0, nullptr, 0);
-  emit_gn_split(p + ".out", h, p + ".out_layers.0", true, SPLIT_SAME, A, ss_all_ + ss_off_.at(p), ss_total_);
-  if (skip) {
-    DDNM_CHECK(!down, "skip convolution on a down block");
-    TcWeights w2 = prep_weights(p + ".out_layers.3.weight", Cout, Cout, 9, p + ".skip_connection.weight", Cin);
-    emit_tc(p + ".conv2+skip", A, TAPS_3X3, &Bs, w2, Cout, out, bias_sum(p + ".out_layers.3.bias", p + ".skip_connection.bias", Cout), 0,
-            nullptr, 0);
-  } else {
-    DDNM_CHECK(Cin == Cout, "identity skip needs equal channels");
-    TcWeights w2 = prep_weights(p + ".out_layers.3.weight", Cout, Cout, 9, "", 0);
-    emit_tc(p + ".conv2", A, TAPS_3X3, nullptr, w2, Cout, out, P(p + ".out_layers.3.bias", Cout), 0, x.p, x.ld, down ? 2 : 0);
-  }
-  rec.kind = 0;
-  rec.r = Res{p, x, h, out, down, skip};
-}
-
-// AttentionBlock._forward (unet.py:299-305), QKVAttentionLegacy; qkv kept in its own buffer
-void UNetEncoder::emit_attn(const std::string& p, const View& x, const View& out, Layer& rec) {
-  const int C = x.C, T = x.H * x.W, ch = cfg_.num_head_channels, heads = C / ch;
-  DDNM_CHECK(C % ch == 0, "channels not divisible by num_head_channels");
-  SplitView A{splitA_hi_, splitA_lo_};
-  emit_gn_split(p + ".norm", x, p + ".norm", false, SPLIT_SAME, A);
-  TcWeights wqkv = prep_weights(p + ".qkv.weight", 3 * C, C, 1, "", 0);
-  float* qkvbuf = (float*)arena_.alloc((size_t)B_ * T * 3 * C * 4);
-  View qkv;
-  qkv.p = qkvbuf; qkv.N = B_; qkv.H = x.H; qkv.W = x.W; qkv.C = 3 * C; qkv.ld = 3 * C;
-  emit_tc(p + ".qkv", A, TAPS_1X1, nullptr, wqkv, 3 * C, qkv, P(p + ".qkv.bias", 3 * C), 0, nullptr, 0);
-  float* shared_qkv = qkv_;
-  qkv_ = qkvbuf;   // emit_attention_core reads q | k | v from qkv_
-  emit_attention_core(p, T, heads, ch, 3 * C, 3 * ch, 0, ch, 2 * ch, 1.0f / std::sqrt((float)ch));
-  qkv_ = shared_qkv;
-  View ov;
-  ov.p = attO_; ov.N = B_; ov.H = x.H; ov.W = x.W; ov.C = C; ov.ld = C;
-  emit_gn_split(p + ".proj_in", ov, "", false, SPLIT_SAME, A);
-  TcWeights wp = prep_weights(p + ".proj_out.weight", C, C, 1, "", 0);
-  emit_tc(p + ".proj_out", A, TAPS_1X1, nullptr, wp, C, out, P(p + ".proj_out.bias", C), 0, x.p, x.ld);
-  rec.kind = 1;
-  rec.a = Attn{p, x, out, qkvbuf};
-}
-
 // self.out (unet.py:853-871): GroupNorm + SiLU, then AttentionPool2d (unet.py:20-50) or mean + 1x1 convolution
 void UNetEncoder::emit_head(const View& h) {
   const int C = h.C, HW = h.H * h.W, O = cfg_.out_channels, Bn = B_;
@@ -580,11 +531,6 @@ void UNetEncoder::emit_backward(const View& stem_out, const std::vector<Layer>& 
   const int Bn = B_, O = cfg_.out_channels;
   SplitView SA{splitA_hi_, splitA_lo_}, SB{splitB_hi_, splitB_lo_};
   float* G[2] = {gx_[0], gx_[1]};
-  auto grad_view = [&](float* p, int H, int W, int C) {
-    View v;
-    v.p = p; v.N = Bn; v.H = H; v.W = W; v.C = C; v.ld = C;
-    return v;
-  };
   auto with_dims = [](SplitView s, const View& v) {
     s.N = v.N; s.H = v.H; s.W = v.W; s.C = v.C;
     return s;
@@ -628,26 +574,26 @@ void UNetEncoder::emit_backward(const View& stem_out, const std::vector<Layer>& 
       const int Cin = r.x.C, Cout = r.out.C;
       const SplitView sb = with_dims(SB, r.out);
       TcWeights w2 = prep_weights_t(r.p + ".out_layers.3.weight", Cout, Cout, 9);
-      emit_tc(r.p + ".conv2.dgrad", sb, TAPS_3X3, nullptr, w2, Cout, grad_view(g1_, r.out.H, r.out.W, Cout), nullptr, 0, nullptr, 0);
+      emit_tc(r.p + ".conv2.dgrad", sb, TAPS_3X3, nullptr, w2, Cout, view_of(g1_, r.out.H, r.out.W, Cout), nullptr, 0, nullptr, 0);
       const float* add = G[0];
       bool add_pool = r.down;
       if (r.skip_conv) {
         TcWeights ws = prep_weights_t(r.p + ".skip_connection.weight", Cout, Cin, 1);
-        emit_tc(r.p + ".skip.dgrad", sb, TAPS_1X1, nullptr, ws, Cin, grad_view(g2_, r.x.H, r.x.W, Cin), nullptr, 0, nullptr, 0);
+        emit_tc(r.p + ".skip.dgrad", sb, TAPS_1X1, nullptr, ws, Cin, view_of(g2_, r.x.H, r.x.W, Cin), nullptr, 0, nullptr, 0);
         add = g2_;
         add_pool = false;
       }
-      emit_gn_backward(r.p + ".out_norm.bwd", g1_, r.h, r.p + ".out_layers.0", ss_all_ + ss_off_.at(r.p), ss_total_, true, false, nullptr,
+      emit_gn_backward(r.p + ".out_norm.bwd", g1_, r.h, r.p + ".out_layers.0", emb_rows(r.p), emb_ld_, true, false, nullptr,
                        false, nullptr, SA);
       TcWeights w1 = prep_weights_t(r.p + ".in_layers.2.weight", Cout, Cin, 9);
-      emit_tc(r.p + ".conv1.dgrad", with_dims(SA, r.h), TAPS_3X3, nullptr, w1, Cin, grad_view(g1_, r.out.H, r.out.W, Cin), nullptr, 0,
+      emit_tc(r.p + ".conv1.dgrad", with_dims(SA, r.h), TAPS_3X3, nullptr, w1, Cin, view_of(g1_, r.out.H, r.out.W, Cin), nullptr, 0,
               nullptr, 0);
       emit_gn_backward(r.p + ".in_norm.bwd", g1_, r.x, r.p + ".in_layers.0", nullptr, 0, true, r.down, add, add_pool, G[1], SB);
     } else {
       const Attn& a = L.a;
       const int C = a.x.C, T = a.x.H * a.x.W, ch = cfg_.num_head_channels, heads = C / ch;
       TcWeights wp = prep_weights_t(a.p + ".proj_out.weight", C, C, 1);
-      emit_tc(a.p + ".proj_out.dgrad", with_dims(SB, a.out), TAPS_1X1, nullptr, wp, C, grad_view(g1_, a.x.H, a.x.W, C), nullptr, 0, nullptr, 0);
+      emit_tc(a.p + ".proj_out.dgrad", with_dims(SB, a.out), TAPS_1X1, nullptr, wp, C, view_of(g1_, a.x.H, a.x.W, C), nullptr, 0, nullptr, 0);
       {
         const float *qkv = a.qkv, *dA = g1_;
         float *Pm = sP_, *dP = sdP_, *dq = gqkv_;
@@ -668,11 +614,11 @@ void UNetEncoder::emit_backward(const View& stem_out, const std::vector<Layer>& 
           bgemm(Bn, heads, T, ch, T, alpha, dP, 1, T, heads * hs, hs, qkv, q3, 1, img, 3 * ch, dq + ch, q3, img, 3 * ch, nullptr, s);
         });
       }
-      View gq = grad_view(gqkv_, a.x.H, a.x.W, 3 * C);
+      View gq = view_of(gqkv_, a.x.H, a.x.W, 3 * C);
       SplitView sq = SA;
       emit_gn_split(a.p + ".dqkv.split", gq, "", false, SPLIT_SAME, sq);
       TcWeights wq = prep_weights_t(a.p + ".qkv.weight", 3 * C, C, 1);
-      emit_tc(a.p + ".qkv.dgrad", sq, TAPS_1X1, nullptr, wq, C, grad_view(g1_, a.x.H, a.x.W, C), nullptr, 0, nullptr, 0);
+      emit_tc(a.p + ".qkv.dgrad", sq, TAPS_1X1, nullptr, wq, C, view_of(g1_, a.x.H, a.x.W, C), nullptr, 0, nullptr, 0);
       emit_gn_backward(a.p + ".norm.bwd", g1_, a.x, a.p + ".norm", nullptr, 0, false, false, G[0], false, G[1], SB);
     }
     std::swap(G[0], G[1]);
@@ -694,64 +640,39 @@ void UNetEncoder::emit_backward(const View& stem_out, const std::vector<Layer>& 
 
 void UNetEncoder::build_program() {
   const EncoderCfg& c = cfg_;
-  const int mc = c.model_channels, R = c.image_size, nrb = c.num_res_blocks, L = c.n_levels;
+  const int mc = c.model_channels, R = c.image_size, L = c.n_levels;
   DDNM_CHECK(mc % 64 == 0, "model_channels must be a multiple of 64 (tensor-core K blocks)");
   DDNM_CHECK(L >= 1 && L <= 8 && R % (1 << (L - 1)) == 0, "image size not divisible by the downsampling");
-  auto attn_at = [&](int ds) {
-    for (int i = 0; i < c.n_attn_ds; ++i)
-      if (c.attn_ds[i] == ds) return true;
-    return false;
-  };
+  for (int lv = 0; lv < L; ++lv) {
+    const int co = c.channel_mult[lv] * mc;
+    DDNM_CHECK(co % 64 == 0 && co > 0, "channel counts must be multiples of 64");
+  }
+  const Torso t = plan_torso(R, c.in_channels, mc, c.channel_mult, L, c.num_res_blocks, c.attn_ds, c.n_attn_ds);
   // ---- sizing: widest activation (incl. qkv rows), attention score matrices, ResBlock scale|shift rows ----
   size_t act_max = (size_t)B_ * R * R * c.channel_mult[0] * mc, att_qkv = 1, att_S = 1, att_O = 1;
-  std::vector<std::string> rb_names;
-  std::vector<int> rb_cout;
-  {
-    int ch = c.channel_mult[0] * mc, res = R, ds = 1, blk = 1;
-    auto attn_plan = [&](int C, int r) {
-      const size_t T = (size_t)r * r, heads = C / c.num_head_channels;
-      act_max = std::max(act_max, (size_t)B_ * T * 3 * C);
-      att_qkv = std::max(att_qkv, (size_t)B_ * T * 3 * C);
-      att_S = std::max(att_S, (size_t)B_ * heads * T * T);
-      att_O = std::max(att_O, (size_t)B_ * T * C);
-    };
-    for (int lv = 0; lv < L; ++lv) {
-      const int co = c.channel_mult[lv] * mc;
-      DDNM_CHECK(co % 64 == 0 && co > 0, "channel counts must be multiples of 64");
-      for (int i = 0; i < nrb; ++i) {
-        act_max = std::max(act_max, (size_t)B_ * res * res * std::max(ch, co));
-        rb_names.push_back("input_blocks." + std::to_string(blk) + ".0");
-        rb_cout.push_back(co);
-        ch = co;
-        if (attn_at(ds)) attn_plan(ch, res);
-        ++blk;
-      }
-      if (lv != L - 1) {
-        rb_names.push_back("input_blocks." + std::to_string(blk) + ".0");
-        rb_cout.push_back(ch);
-        res /= 2;
-        ds *= 2;
-        ++blk;
+  std::vector<EmbProj> projs;
+  auto size_block = [&](const std::string& prefix, const Block& b) {
+    const int r = b.res_in;
+    for (size_t j = 0; j < b.layers.size(); ++j) {
+      const Block::Layer& l = b.layers[j];
+      const std::string p = prefix + "." + std::to_string(j);
+      if (l.kind == LAYER_ATTN) {
+        const size_t T = (size_t)r * r, heads = l.cin / c.num_head_channels;
+        act_max = std::max(act_max, (size_t)B_ * T * 3 * l.cin);
+        att_qkv = std::max(att_qkv, (size_t)B_ * T * 3 * l.cin);
+        att_S = std::max(att_S, (size_t)B_ * heads * T * T);
+        att_O = std::max(att_O, (size_t)B_ * T * l.cin);
+      } else {
+        if (l.kind == LAYER_RES) act_max = std::max(act_max, (size_t)B_ * r * r * std::max(l.cin, l.cout));
+        projs.push_back({p, p + ".emb_layers.1.weight", P(p + ".emb_layers.1.bias", 2 * l.cout), 2 * l.cout});
       }
     }
-    rb_names.push_back("middle_block.0");
-    rb_cout.push_back(ch);
-    rb_names.push_back("middle_block.2");
-    rb_cout.push_back(ch);
-    attn_plan(ch, res);
-    headT_ = res * res + 1;
-  }
+  };
+  for (size_t i = 1; i < t.input.size(); ++i) size_block("input_blocks." + std::to_string(i), t.input[i]);
+  size_block("middle_block", t.middle);
+  headT_ = t.middle.res_in * t.middle.res_in + 1;
+  alloc_common(act_max, 0);
   alloc_attention(att_qkv, att_S, att_O);
-  split_elems_ = act_max;
-  splitA_hi_ = (__half*)arena_.alloc(act_max * 2);
-  splitA_lo_ = (__half*)arena_.alloc(act_max * 2);
-  splitB_hi_ = (__half*)arena_.alloc(act_max * 2);
-  splitB_lo_ = (__half*)arena_.alloc(act_max * 2);
-  x_in_ = (float*)arena_.alloc((size_t)B_ * in_ch_ * R * R * 4);
-  t_in_ = (float*)arena_.alloc((size_t)B_ * 4);
-  labels_in_ = (int*)arena_.alloc((size_t)B_ * 4);
-  CUDA_CHECK(cudaMemset(labels_in_, 0, (size_t)B_ * 4));
-  out_ = (float*)arena_.alloc(out_elems() * 4);
   scale_in_ = (float*)arena_.alloc(4);
   fill_f32_kernel<<<1, 32>>>(scale_in_, 1, 1.0f);   // the scale of an eager profile run before any grad() call
   CUDA_CHECK(cudaGetLastError());
@@ -765,69 +686,39 @@ void UNetEncoder::build_program() {
   gnb_part_elems_ = (size_t)(invariant_ ? B_ * (kGnbInvariantChunks + 1) : 4 * num_sms_ + 2 * B_) * 512 * 2;
   gnb_part_ = (float*)arena_.alloc(gnb_part_elems_ * sizeof(double));
 
-  // ---- timestep embedding and every emb_layers Linear as one matrix (as UNetOpenAI) ----
-  const int tdim = mc * 4;
-  emb_ = (float*)arena_.alloc((size_t)B_ * mc * 4);
-  temb0_ = (float*)arena_.alloc((size_t)B_ * tdim * 4);
-  temb_ = (float*)arena_.alloc((size_t)B_ * tdim * 4);
-  freq_ = (float*)arena_.alloc((size_t)(mc / 2) * 4);
-  CUDA_CHECK(cudaMemcpy(freq_, P("__freq", mc / 2), (mc / 2) * 4, cudaMemcpyDeviceToDevice));
-  ss_total_ = 0;
-  for (size_t i = 0; i < rb_names.size(); ++i) {
-    ss_off_[rb_names[i]] = ss_total_;
-    ss_total_ += 2 * rb_cout[i];
-  }
-  embW_all_ = (float*)arena_.alloc((size_t)ss_total_ * tdim * 4);
-  embB_all_ = (float*)arena_.alloc((size_t)ss_total_ * 4);
-  ss_all_ = (float*)arena_.alloc((size_t)B_ * ss_total_ * 4);
-  for (size_t i = 0; i < rb_names.size(); ++i) {
-    const int off = ss_off_[rb_names[i]], n2 = 2 * rb_cout[i];
-    CUDA_CHECK(cudaMemcpy(embW_all_ + (size_t)off * tdim, P(rb_names[i] + ".emb_layers.1.weight", (long long)n2 * tdim), (size_t)n2 * tdim * 4,
-                          cudaMemcpyDeviceToDevice));
-    CUDA_CHECK(cudaMemcpy(embB_all_ + off, P(rb_names[i] + ".emb_layers.1.bias", n2), (size_t)n2 * 4, cudaMemcpyDeviceToDevice));
-  }
-  {
-    float *t = t_in_, *emb = emb_, *t0 = temb0_, *t1 = temb_, *fr = freq_, *ss = ss_all_, *W = embW_all_, *Bv = embB_all_;
-    const float *w0 = P("time_embed.0.weight", (long long)tdim * mc), *b0 = P("time_embed.0.bias", tdim);
-    const float *w1 = P("time_embed.2.weight", (long long)tdim * tdim), *b1 = P("time_embed.2.bias", tdim);
-    const int Bn = B_, mcn = mc, tot = ss_total_;
-    add_op("time_embed", "temb", 0, 0, [=](cudaStream_t s) {
-      sinusoid(t, Bn, fr, mcn, false, emb, s);
-      linear(emb, Bn, mcn, w0, b0, tdim, t0, tdim, 0, 1, s);
-      linear(t0, Bn, tdim, w1, b1, tdim, t1, tdim, 0, 1, s);
-      linear(t1, Bn, tdim, W, Bv, tot, ss, tot, 0, 0, s);
-    });
-  }
+  emit_time_embed("time_embed", "time_embed.0", "time_embed.2", mc, false, nullptr, 0, projs);
 
-  // ---- torso ----
+  // ---- torso: every ResBlock and AttentionBlock keeps its activations for the backward pass ----
   std::vector<Layer> layers;
   View h = new_view(R, R, c.channel_mult[0] * mc);
   emit_stem("input_blocks.0.0", h);
   const View stem_out = h;
-  int ds = 1, blk = 1;
-  auto run = [&](const std::string& p, int kind, int cout, int ro) {
-    View dst = new_view(ro, ro, cout);
-    Layer rec;
-    if (kind == 2) emit_attn(p, h, dst, rec);
-    else emit_resblock(p, h, dst, kind == 1, rec);
-    layers.push_back(rec);
-    h = dst;
+  auto run_block = [&](const std::string& prefix, const Block& b) {
+    for (size_t j = 0; j < b.layers.size(); ++j) {
+      const Block::Layer& l = b.layers[j];
+      const std::string p = prefix + "." + std::to_string(j);
+      const int ro = l.kind == LAYER_RES_DOWN ? h.H / 2 : h.H;
+      View dst = new_view(ro, ro, l.cout);
+      Layer rec;
+      if (l.kind == LAYER_ATTN) {
+        // QKVAttentionLegacy; the qkv rows in a buffer of their own
+        DDNM_CHECK(h.C % c.num_head_channels == 0, "channels not divisible by num_head_channels");
+        float* qkv = (float*)arena_.alloc((size_t)B_ * h.H * h.W * 3 * h.C * 4);
+        emit_attention_block(p, h, dst, h.C / c.num_head_channels, false, qkv);
+        rec.kind = 1;
+        rec.a = Attn{p, h, dst, qkv};
+      } else {
+        View hv = new_view(ro, ro, l.cout);
+        emit_res_block(p, h, hv, dst, l.kind);
+        rec.kind = 0;
+        rec.r = Res{p, h, hv, dst, l.kind == LAYER_RES_DOWN, has_param(p + ".skip_connection.weight")};
+      }
+      layers.push_back(rec);
+      h = dst;
+    }
   };
-  for (int lv = 0; lv < L; ++lv) {
-    const int co = c.channel_mult[lv] * mc;
-    for (int i = 0; i < nrb; ++i) {
-      const std::string p = "input_blocks." + std::to_string(blk++);
-      run(p + ".0", 0, co, h.H);
-      if (attn_at(ds)) run(p + ".1", 2, co, h.H);
-    }
-    if (lv != L - 1) {
-      run("input_blocks." + std::to_string(blk++) + ".0", 1, h.C, h.H / 2);
-      ds *= 2;
-    }
-  }
-  run("middle_block.0", 0, h.C, h.H);
-  run("middle_block.1", 2, h.C, h.H);
-  run("middle_block.2", 0, h.C, h.H);
+  for (size_t i = 1; i < t.input.size(); ++i) run_block("input_blocks." + std::to_string(i), t.input[i]);
+  run_block("middle_block", t.middle);
   hf_ = (float*)arena_.alloc((size_t)B_ * h.H * h.W * h.C * 4);
   tok_ = (float*)arena_.alloc((size_t)B_ * headT_ * h.C * 4);
   hqkv_ = (float*)arena_.alloc((size_t)B_ * headT_ * 3 * h.C * 4);

@@ -1,4 +1,4 @@
-// UNetEngine: what the two denoiser programs share — parameters, arena, scratch, op emitters, CUDA-graph replay.
+// UNetEngine: what the three programs share — parameters, arena, scratch, op emitters, CUDA-graph replay.
 //
 // Data layout in HBM: activations fp32 NHWC; every skip tensor is born inside the channel slice of the concat
 // buffer its up-path consumer will read (torch.cat at models.py:331 / unet.py:661 costs nothing); the tensor-core
@@ -71,11 +71,15 @@ const float* UNetEngine::P(const std::string& name, long long expect) const {
 }
 
 View UNetEngine::new_view(int H, int W, int C) {
-  View v;
-  v.N = B_; v.H = H; v.W = W; v.C = C; v.ld = C;
-  v.p = (float*)arena_.alloc((size_t)B_ * H * W * C * sizeof(float));
+  View v = view_of((float*)arena_.alloc((size_t)B_ * H * W * C * sizeof(float)), H, W, C);
   v.st = new_stats(C);
   v.st_ld = C;
+  return v;
+}
+
+View UNetEngine::view_of(float* p, int H, int W, int C) const {
+  View v;
+  v.p = p; v.N = B_; v.H = H; v.W = W; v.C = C; v.ld = C;
   return v;
 }
 
@@ -178,8 +182,7 @@ void UNetEngine::emit_tc(const std::string& name, const SplitView& a, int mode, 
   if (S > 1) {
     const long long stride = out.pixels() * Cout;
     float* part = (float*)arena_.alloc((size_t)S * stride * sizeof(float));
-    View pv;
-    pv.p = part; pv.N = out.N; pv.H = out.H; pv.W = out.W; pv.C = Cout; pv.ld = Cout;
+    const View pv = view_of(part, out.H, out.W, Cout);
     TcLaunch Ls = tc_make_launch(a, mode, side, w.hi, w.lo, 1, Cout, pv, nullptr, 0, nullptr, 0, 1.0f, num_sms_, 0, invariant_);
     DDNM_CHECK(Ls.BN == L.BN, "split-K: tile shape changed");
     Ls.p.split_k = S;
@@ -202,12 +205,12 @@ void UNetEngine::alloc_common(size_t split_elems, size_t hbuf_elems) {
   splitA_lo_ = (__half*)arena_.alloc(split_elems * 2);
   splitB_hi_ = (__half*)arena_.alloc(split_elems * 2);
   splitB_lo_ = (__half*)arena_.alloc(split_elems * 2);
-  hbuf_ = (float*)arena_.alloc(hbuf_elems * 4);
+  if (hbuf_elems) hbuf_ = (float*)arena_.alloc(hbuf_elems * 4);
   x_in_ = (float*)arena_.alloc((size_t)B_ * in_ch_ * R_ * R_ * 4);
   t_in_ = (float*)arena_.alloc((size_t)B_ * 4);
   labels_in_ = (int*)arena_.alloc((size_t)B_ * 4);
   CUDA_CHECK(cudaMemset(labels_in_, 0, (size_t)B_ * 4));
-  out_ = (float*)arena_.alloc((size_t)B_ * out_ch_ * R_ * R_ * 4);
+  out_ = (float*)arena_.alloc(out_elems() * 4);
   if (lowres_ > 0) lowres_in_ = (float*)arena_.alloc((size_t)B_ * in_ch_ * lowres_ * lowres_ * 4);
 }
 
@@ -238,9 +241,9 @@ void UNetEngine::alloc_attention(size_t qkv_elems, size_t s_elems, size_t o_elem
   vtl_ = (__half*)arena_.alloc(o_elems * 2);
 }
 
-void UNetEngine::emit_attention_core(const std::string& name, int T, int heads, int ch, int qkv_ld, int head_stride, int q_off,
-                                     int k_off, int v_off, float alpha) {
-  float *q = qkv_, *S = attS_, *O = attO_;
+void UNetEngine::emit_attention_core(const std::string& name, float* qkv, int T, int heads, int ch, int qkv_ld, int head_stride,
+                                     int q_off, int k_off, int v_off, float alpha) {
+  float *q = qkv, *S = attS_, *O = attO_;
   const int Bn = B_, C = heads * ch;
   const long long img = (long long)T * qkv_ld;
   const double fl = 2.0 * Bn * heads * (double)T * T * ch;
@@ -252,8 +255,7 @@ void UNetEngine::emit_attention_core(const std::string& name, int T, int heads, 
     __half *qh = qkvh_, *ql = qkvl_, *ph = ph_, *pl = pl_, *vh = vth_, *vl = vtl_;
     // the raw split is elementwise, so the [token][qkv_ld] buffer is viewed as rows of C = heads*ch channels (<= MAX_C)
     DDNM_CHECK(qkv_ld % C == 0, "qkv row is not a multiple of the attention width");
-    View qv;
-    qv.p = qkv_; qv.N = B_; qv.H = 1; qv.W = T * (qkv_ld / C); qv.C = C; qv.ld = C;
+    const View qv = view_of(qkv, 1, T * (qkv_ld / C), C);
     add_op(name + ".qkv_split", "gn_split", 0, (double)Bn * T * qkv_ld * 8,
            [=](cudaStream_t s) { gn_apply_split(qv, 1, false, nullptr, nullptr, 0.f, false, SPLIT_SAME, qh, ql, s); });
     const long long hs = head_stride ? head_stride : qkv_ld;   // extent-1 dims still need a legal (non-zero) TMA stride
@@ -332,13 +334,128 @@ void UNetEngine::emit_head(const std::string& norm, const std::string& conv, con
   std::vector<float> hb(64, 0.f);
   CUDA_CHECK(cudaMemcpy(hb.data(), P(conv + ".bias", out_ch_), out_ch_ * sizeof(float), cudaMemcpyDeviceToHost));
   float* bias64 = dev_copy(hb);
-  View o64;
-  o64.N = B_; o64.H = fh.H; o64.W = fh.W; o64.C = 64; o64.ld = 64;
-  o64.p = (float*)arena_.alloc((size_t)B_ * fh.H * fh.W * 64 * sizeof(float));
+  const View o64 = view_of((float*)arena_.alloc((size_t)B_ * fh.H * fh.W * 64 * sizeof(float)), fh.H, fh.W, 64);
   emit_tc("head.conv", A, TAPS_3X3, nullptr, w, 64, o64, bias64, 0, nullptr, 0);
   float* o = out_;
   const View real = o64.slice(0, out_ch_);
   add_op("head.to_nchw", "head", 0, (double)fh.pixels() * (64 + out_ch_) * 4, [=](cudaStream_t s) { nhwc_to_nchw(real, o, s); });
+}
+
+// timestep embedding (models.py:6-24,305-308 / nn.py:103-121, unet.py:472-479,649-653) and every block's projection of it
+// (models.py:121 temb_proj / unet.py:188-194 emb_layers) as one matrix, so one Linear computes the rows of all blocks
+void UNetEngine::emit_time_embed(const std::string& name, const std::string& layer0, const std::string& layer1, int ch,
+                                 bool sin_first, const float* label_emb, int num_classes, const std::vector<EmbProj>& projs) {
+  const int tdim = ch * 4;
+  float* emb = (float*)arena_.alloc((size_t)B_ * ch * 4);
+  float* t0 = (float*)arena_.alloc((size_t)B_ * tdim * 4);
+  float* t1 = (float*)arena_.alloc((size_t)B_ * tdim * 4);
+  float* fr = (float*)arena_.alloc((size_t)(ch / 2) * 4);
+  CUDA_CHECK(cudaMemcpy(fr, P("__freq", ch / 2), (ch / 2) * 4, cudaMemcpyDeviceToDevice));
+  emb_ld_ = 0;
+  for (const EmbProj& pr : projs) {
+    emb_off_[pr.block] = emb_ld_;
+    emb_ld_ += pr.rows;
+  }
+  float* W = (float*)arena_.alloc((size_t)emb_ld_ * tdim * 4);
+  float* Bv = (float*)arena_.alloc((size_t)emb_ld_ * 4);
+  emb_all_ = (float*)arena_.alloc((size_t)B_ * emb_ld_ * 4);
+  for (const EmbProj& pr : projs) {
+    const int off = emb_off_[pr.block];
+    CUDA_CHECK(cudaMemcpy(W + (size_t)off * tdim, P(pr.weight, (long long)pr.rows * tdim), (size_t)pr.rows * tdim * 4,
+                          cudaMemcpyDeviceToDevice));
+    CUDA_CHECK(cudaMemcpy(Bv + off, pr.bias, (size_t)pr.rows * 4, cudaMemcpyDeviceToDevice));
+  }
+  const float *w0 = P(layer0 + ".weight", (long long)tdim * ch), *b0 = P(layer0 + ".bias", tdim);
+  const float *w1 = P(layer1 + ".weight", (long long)tdim * tdim), *b1 = P(layer1 + ".bias", tdim);
+  const float* t = t_in_;
+  const int* labels = labels_in_;
+  float* rows = emb_all_;
+  const int Bn = B_, tot = emb_ld_;
+  add_op(name, "temb", 0, 0, [=](cudaStream_t s) {
+    sinusoid(t, Bn, fr, ch, sin_first, emb, s);
+    // every block consumes the embedding through a SiLU (models.py:121, unet.py:190), so the activations are applied once at the
+    // producers' outputs
+    linear(emb, Bn, ch, w0, b0, tdim, t0, tdim, 0, 1, s);
+    if (label_emb) {
+      linear(t0, Bn, tdim, w1, b1, tdim, t1, tdim, 0, 0, s);
+      add_label_swish(t1, label_emb, labels, Bn, tdim, num_classes, s);   // t1 = SiLU(emb + label_emb[y])
+    } else {
+      linear(t0, Bn, tdim, w1, b1, tdim, t1, tdim, 0, 1, s);
+    }
+    linear(t1, Bn, tdim, W, Bv, tot, rows, tot, 0, 0, s);
+  });
+}
+
+UNetEngine::Torso UNetEngine::plan_torso(int image_size, int in_channels, int model_channels, const int* channel_mult, int n_levels,
+                                         int num_res_blocks, const int* attn_ds, int n_attn_ds) {
+  auto attn_at = [&](int ds) { return std::find(attn_ds, attn_ds + n_attn_ds, ds) != attn_ds + n_attn_ds; };
+  Torso t;
+  int ch = channel_mult[0] * model_channels, ds = 1, res = image_size;
+  t.input.push_back({{{LAYER_CONV, in_channels, ch}}, res, res, ch});
+  for (int lv = 0; lv < n_levels; ++lv) {
+    const int co = channel_mult[lv] * model_channels;
+    for (int i = 0; i < num_res_blocks; ++i) {
+      Block b{{{LAYER_RES, ch, co}}, res, res, co};
+      ch = co;
+      if (attn_at(ds)) b.layers.push_back({LAYER_ATTN, ch, ch});
+      t.input.push_back(b);
+    }
+    if (lv != n_levels - 1) {
+      t.input.push_back({{{LAYER_RES_DOWN, ch, ch}}, res, res / 2, ch});
+      res /= 2;
+      ds *= 2;
+    }
+  }
+  t.middle = {{{LAYER_RES, ch, ch}, {LAYER_ATTN, ch, ch}, {LAYER_RES, ch, ch}}, res, res, ch};
+  return t;
+}
+
+//   LAYER_RES_DOWN: h = avg_pool(SiLU(GN(x))), x = avg_pool(x);  LAYER_RES_UP: nearest x2 of both (h_upd / x_upd, :170-177)
+void UNetEngine::emit_res_block(const std::string& p, const View& x, const View& h, const View& out, int kind) {
+  const int Cin = x.C, Cout = out.C;
+  if (kind != LAYER_RES) DDNM_CHECK(Cin == Cout, "up/down ResBlocks keep the channel count");
+  SplitView A{splitA_hi_, splitA_lo_}, Bs{splitB_hi_, splitB_lo_};
+  const int mode1 = kind == LAYER_RES_DOWN ? SPLIT_AVG2 : SPLIT_SAME;
+  const bool has_skip_conv = has_param(p + ".skip_connection.weight");
+  emit_gn_split(p + ".in", x, p + ".in_layers.0", true, mode1, A, nullptr, 0, has_skip_conv ? &Bs : nullptr);
+  if (kind == LAYER_RES_UP) {
+    // in_conv(nearest_up(SiLU(GN(x)))) as four 2x2 parity-phase convolutions on the low-res activation
+    emit_up2_conv(p + ".conv1", A, p + ".in_layers.2.weight", Cout, h, P(p + ".in_layers.2.bias", Cout), 0);
+  } else {
+    TcWeights w1 = prep_weights(p + ".in_layers.2.weight", Cout, Cin, 9, "", 0);
+    emit_tc(p + ".conv1", A, TAPS_3X3, nullptr, w1, Cout, h, P(p + ".in_layers.2.bias", Cout), 0, nullptr, 0);
+  }
+  // out_norm(h) * (1 + scale) + shift -> SiLU -> conv  (:250-253); scale|shift = emb_layers(emb) computed once per forward
+  emit_gn_split(p + ".out", h, p + ".out_layers.0", true, SPLIT_SAME, A, emb_rows(p), emb_ld_);
+  if (has_skip_conv) {
+    DDNM_CHECK(kind == LAYER_RES, "skip convolution on an up/down block");
+    TcWeights w2 = prep_weights(p + ".out_layers.3.weight", Cout, Cout, 9, p + ".skip_connection.weight", Cin);
+    emit_tc(p + ".conv2+skip", A, TAPS_3X3, &Bs, w2, Cout, out, bias_sum(p + ".out_layers.3.bias", p + ".skip_connection.bias", Cout), 0,
+            nullptr, 0);
+  } else {
+    DDNM_CHECK(Cin == Cout, "identity skip needs equal channels");
+    TcWeights w2 = prep_weights(p + ".out_layers.3.weight", Cout, Cout, 9, "", 0);
+    emit_tc(p + ".conv2", A, TAPS_3X3, nullptr, w2, Cout, out, P(p + ".out_layers.3.bias", Cout), 0, x.p, x.ld,
+            kind == LAYER_RES_UP ? 1 : (kind == LAYER_RES_DOWN ? 2 : 0));
+  }
+}
+
+// weight = softmax((q*s)^T (k*s)), s = ch^-1/4; a = weight . v; head h of a is channels [h*ch, (h+1)*ch) in both orders.  The qkv
+// channels of head h are
+//   QKVAttentionLegacy (:337-354): [q | k | v] at h*3ch + {0, ch, 2ch}   (heads split before q, k, v)
+//   QKVAttention (:361-389):       h*ch + {0, C, 2C}                    (q, k, v split before the heads; new_order)
+void UNetEngine::emit_attention_block(const std::string& p, const View& x, const View& out, int heads, bool new_order, float* qkv) {
+  const int C = x.C, T = x.H * x.W, ch = C / heads;
+  SplitView A{splitA_hi_, splitA_lo_};
+  emit_gn_split(p + ".norm", x, p + ".norm", false, SPLIT_SAME, A);
+  TcWeights wqkv = prep_weights(p + ".qkv.weight", 3 * C, C, 1, "", 0);
+  emit_tc(p + ".qkv", A, TAPS_1X1, nullptr, wqkv, 3 * C, view_of(qkv, x.H, x.W, 3 * C), P(p + ".qkv.bias", 3 * C), 0, nullptr, 0);
+  const float alpha = 1.0f / std::sqrt((float)ch);   // (ch^-1/4)^2
+  if (new_order) emit_attention_core(p, qkv, T, heads, ch, 3 * C, ch, 0, C, 2 * C, alpha);
+  else emit_attention_core(p, qkv, T, heads, ch, 3 * C, 3 * ch, 0, ch, 2 * ch, alpha);
+  emit_gn_split(p + ".proj_in", view_of(attO_, x.H, x.W, C), "", false, SPLIT_SAME, A);
+  TcWeights wp = prep_weights(p + ".proj_out.weight", C, C, 1, "", 0);
+  emit_tc(p + ".proj_out", A, TAPS_1X1, nullptr, wp, C, out, P(p + ".proj_out.bias", C), 0, x.p, x.ld);
 }
 
 void UNetEngine::set_terms(int t) {

@@ -1,6 +1,7 @@
-// The denoiser engines: static launch programs for the two UNets on the reference's hot path
-//   UNetSimple  <- guided_diffusion/models.py::Model      (celeba_hq.yml, model.type == "simple")
-//   UNetOpenAI  <- guided_diffusion/unet.py::UNetModel    (imagenet_256.yml, model.type == "openai")
+// The engines: static launch programs for the three networks on the reference's hot path
+//   UNetSimple   <- guided_diffusion/models.py::Model             (celeba_hq.yml, model.type == "simple")
+//   UNetOpenAI   <- guided_diffusion/unet.py::UNetModel           (imagenet_256.yml, model.type == "openai")
+//   UNetEncoder  <- guided_diffusion/unet.py::EncoderUNetModel    (the classifier of imagenet_256_cc.yml)
 // built once per (config, batch) and replayed as a CUDA graph.  UNetEngine holds everything they share.
 #pragma once
 #include <functional>
@@ -102,6 +103,8 @@ class UNetEngine {
   struct Param { float* p; long long n; };
   const float* P(const std::string& name, long long expect = -1) const;
   View new_view(int H, int W, int C);
+  // [B_][H][W][C] over existing memory, no statistics
+  View view_of(float* p, int H, int W, int C) const;
   StatAcc* new_stats(int C);
   struct TcWeights { __half *hi, *lo; int ktot; };
   // main / side: full parameter names of the OIHW weight tensors ("" = absent)
@@ -118,12 +121,12 @@ class UNetEngine {
                      const float* ss = nullptr, int ss_ld = 0, SplitView* raw = nullptr);
   void emit_tc(const std::string& name, const SplitView& a, int mode, const SplitView* side, const TcWeights& w, int Cout,
                const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int res_mode = 0);
-  // softmax(alpha * Q K^T) V for `heads` heads of width ch over T tokens; q/k/v live in the fp32 qkv_ buffer
+  // softmax(alpha * Q K^T) V for `heads` heads of width ch over T tokens; q/k/v live in the fp32 buffer qkv
   // ([token][qkv_ld], head h at column h*head_stride + {q_off, k_off, v_off}); result -> attO_ [token][heads*ch].
   // T % 128 == 0 and ch % 8 == 0 run both contractions on the tensor cores (a head width that is not a multiple of 64 ends in a
   // zero-filled partial k-block / N tile), otherwise (8x8 maps) on CUDA cores.
-  void emit_attention_core(const std::string& name, int T, int heads, int ch, int qkv_ld, int head_stride, int q_off, int k_off,
-                           int v_off, float alpha);
+  void emit_attention_core(const std::string& name, float* qkv, int T, int heads, int ch, int qkv_ld, int head_stride, int q_off,
+                           int k_off, int v_off, float alpha);
   void alloc_attention(size_t qkv_elems, size_t s_elems, size_t o_elems);
   // conv3x3(nearest_upsample_x2(a)) + bias as 4 parity-phase 2x2 convolutions on the low-res split `a` (4/9 of the MACs,
   // no upsampled copy); wname: OIHW 3x3 weight parameter
@@ -131,6 +134,33 @@ class UNetEngine {
                      const float* chanadd, int ca_ld);
   void emit_stem(const std::string& wname, const View& out);
   void emit_head(const std::string& norm, const std::string& conv, const View& h);
+
+  // one block's projection of the timestep embedding: `rows` rows of the stacked matrix, from the [rows, 4 ch] parameter `weight`
+  struct EmbProj { std::string block, weight; const float* bias; int rows; };
+  // timestep embedding: sinusoid(t) over ch channels ([sin | cos] if sin_first), layer0 -> SiLU -> layer1 (+ label_emb[labels_in_]
+  // if label_emb) -> SiLU, then every projection in `projs` as one stacked Linear into [B][emb_ld_] rows (emb_rows)
+  void emit_time_embed(const std::string& name, const std::string& layer0, const std::string& layer1, int ch, bool sin_first,
+                       const float* label_emb, int num_classes, const std::vector<EmbProj>& projs);
+  const float* emb_rows(const std::string& block) const { return emb_all_ + emb_off_.at(block); }
+
+  // guided_diffusion/unet.py's module lists as data: a block is one TimestepEmbedSequential, its layers run in order
+  enum LayerKind { LAYER_CONV, LAYER_RES, LAYER_RES_DOWN, LAYER_RES_UP, LAYER_ATTN };
+  struct Block {
+    struct Layer { int kind, cin, cout; };
+    std::vector<Layer> layers;
+    int res_in, res_out, cout;
+  };
+  struct Torso { std::vector<Block> input; Block middle; };
+  // input_blocks (input[0] is the stem convolution) and middle_block of UNetModel / EncoderUNetModel (unet.py:482-565, :740-823)
+  static Torso plan_torso(int image_size, int in_channels, int model_channels, const int* channel_mult, int n_levels,
+                          int num_res_blocks, const int* attn_ds, int n_attn_ds);
+  // ResBlock._forward (unet.py:236-256), use_scale_shift_norm = True; kind LAYER_RES, LAYER_RES_DOWN or LAYER_RES_UP.
+  // h: where in_layers' convolution writes (out's shape), with the statistics out_layers' GroupNorm reads
+  void emit_res_block(const std::string& p, const View& x, const View& h, const View& out, int kind);
+  // AttentionBlock._forward (unet.py:299-305); qkv: [B][T][3C] destination of the qkv convolution
+  void emit_attention_block(const std::string& p, const View& x, const View& out, int heads, bool new_order, float* qkv);
+
+  // hbuf_elems == 0: no resblock intermediate
   void alloc_common(size_t split_elems, size_t hbuf_elems);
   virtual void build_program() = 0;
   // elements of the result forward() copies out: [B, out_ch, R, R] for the denoisers
@@ -165,10 +195,9 @@ class UNetEngine {
   __half *qkvh_ = nullptr, *qkvl_ = nullptr, *ph_ = nullptr, *pl_ = nullptr, *vth_ = nullptr, *vtl_ = nullptr;
   struct StatsChunk { StatAcc* p; size_t cap, used; };
   std::vector<StatsChunk> stats_chunks_;
-  float *emb_ = nullptr, *temb0_ = nullptr, *temb_ = nullptr, *ca_all_ = nullptr, *freq_ = nullptr;
-  int ca_total_ = 0;
-  std::map<std::string, int> ca_off_;
-  float *tembW_all_ = nullptr, *tembB_all_ = nullptr;
+  float* emb_all_ = nullptr;   // [B][emb_ld_] every block's projection of the timestep embedding
+  int emb_ld_ = 0;
+  std::map<std::string, int> emb_off_;
   cudaGraph_t graph_ = nullptr;
   cudaGraphExec_t graph_exec_ = nullptr;
 };
@@ -191,17 +220,10 @@ class UNetOpenAI : public UNetEngine {
   UNetOpenAI(const OpenAICfg& cfg, int batch);
 
  private:
-  enum ResKind { RES_PLAIN = 0, RES_DOWN = 1, RES_UP = 2 };
   void build_program() override;
-  void emit_resblock(const std::string& p, const View& x, const View& out, int kind);
   // heads of an attention block over C channels; upsample: the block belongs to the output blocks
   int attn_heads(int C, bool upsample) const;
-  void emit_attn(const std::string& p, const View& x, const View& out, int heads);
   OpenAICfg cfg_;
-  float* ss_all_ = nullptr;     // [B][ss_total_] scale|shift rows of every ResBlock (emb_layers outputs)
-  int ss_total_ = 0;
-  std::map<std::string, int> ss_off_;
-  float *embW_all_ = nullptr, *embB_all_ = nullptr;
 };
 
 // guided_diffusion/unet.py::EncoderUNetModel (the classifier of imagenet_256_cc.yml): use_scale_shift_norm, resblock_updown,
@@ -241,8 +263,6 @@ class UNetEncoder : public UNetEngine {
   struct Res { std::string p; View x, h, out; bool down, skip_conv; };
   struct Attn { std::string p; View x, out; float* qkv; };
   struct Layer { int kind; Res r; Attn a; };   // kind 0 ResBlock, 1 AttentionBlock
-  void emit_resblock(const std::string& p, const View& x, const View& out, bool down, Layer& rec);
-  void emit_attn(const std::string& p, const View& x, const View& out, Layer& rec);
   void emit_head(const View& h);
   void emit_backward(const View& stem_out, const std::vector<Layer>& layers, const View& top);
   // GroupNorm (+ scale-shift) (+ SiLU) (+ 2x2 average pool) backward: g = gradient of the block's activation, x = the
@@ -251,10 +271,6 @@ class UNetEncoder : public UNetEngine {
                         bool silu, bool pool, const float* add, bool add_pool, float* dx32, const SplitView& dst);
   TcWeights prep_weights_t(const std::string& w, int Cout, int Cin, int taps);
   EncoderCfg cfg_;
-  float* ss_all_ = nullptr;
-  int ss_total_ = 0;
-  std::map<std::string, int> ss_off_;
-  float *embW_all_ = nullptr, *embB_all_ = nullptr;
   // head (attention pool): tokens X [B][T][C], qkv [B][T][3C], probabilities [B][heads][T], pooled a0 [B][C]
   int headT_ = 0;
   float *hf_ = nullptr, *tok_ = nullptr, *hqkv_ = nullptr, *hp_ = nullptr, *ha0_ = nullptr;

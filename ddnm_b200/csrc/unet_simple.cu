@@ -15,13 +15,12 @@ void UNetSimple::emit_resblock(const std::string& p, const View& x, const View& 
   const int Cin = x.C, Cout = out.C;
   DDNM_CHECK((size_t)(x.pixels() * Cout) <= hbuf_elems_, "hbuf too small");
   SplitView A{splitA_hi_, splitA_lo_}, Bs{splitB_hi_, splitB_lo_};
-  View h;
-  h.p = hbuf_; h.N = B_; h.H = x.H; h.W = x.W; h.C = Cout; h.ld = Cout;
+  View h = view_of(hbuf_, x.H, x.W, Cout);
   h.st = new_stats(Cout); h.st_ld = Cout;   // conv1's epilogue accumulates the sums norm2 needs
   // blocks with a 1x1 shortcut also need the raw split of x: produced by the same pass that normalises it
   emit_gn_split(p + ".norm1", x, p + ".norm1", true, SPLIT_SAME, A, nullptr, 0, Cin != Cout ? &Bs : nullptr);
   TcWeights w1 = prep_weights(p + ".conv1.weight", Cout, Cin, 9, "", 0);
-  emit_tc(p + ".conv1", A, TAPS_3X3, nullptr, w1, Cout, h, ca_all_ + ca_off_.at(p), ca_total_, nullptr, 0);
+  emit_tc(p + ".conv1", A, TAPS_3X3, nullptr, w1, Cout, h, emb_rows(p), emb_ld_, nullptr, 0);
   emit_gn_split(p + ".norm2", h, p + ".norm2", true, SPLIT_SAME, A);
   if (Cin != Cout) {
     // nin_shortcut (1x1 on the raw block input) rides along as extra K blocks of conv2's GEMM
@@ -51,14 +50,10 @@ void UNetSimple::emit_attn(const std::string& p, const View& x, const View& out)
     CUDA_CHECK(cudaMemcpy(hb.data() + i * C, P(p + nm[i] + ".bias", C), C * sizeof(float), cudaMemcpyDeviceToHost));
   }
   float* bqkv = dev_copy(hb);
-  View qkv;
-  qkv.p = qkv_; qkv.N = B_; qkv.H = x.H; qkv.W = x.W; qkv.C = 3 * C; qkv.ld = 3 * C;
-  emit_tc(p + ".qkv", A, TAPS_1X1, nullptr, wqkv, 3 * C, qkv, bqkv, 0, nullptr, 0);
+  emit_tc(p + ".qkv", A, TAPS_1X1, nullptr, wqkv, 3 * C, view_of(qkv_, x.H, x.W, 3 * C), bqkv, 0, nullptr, 0);
   // one head of width C; w_ = bmm(q, k) * int(c) ** (-0.5)
-  emit_attention_core(p, T, 1, C, 3 * C, 0, 0, C, 2 * C, 1.0f / sqrtf((float)C));
-  View ov;
-  ov.p = attO_; ov.N = B_; ov.H = x.H; ov.W = x.W; ov.C = C; ov.ld = C;
-  emit_gn_split(p + ".proj_in", ov, "", false, SPLIT_SAME, A);
+  emit_attention_core(p, qkv_, T, 1, C, 3 * C, 0, 0, C, 2 * C, 1.0f / sqrtf((float)C));
+  emit_gn_split(p + ".proj_in", view_of(attO_, x.H, x.W, C), "", false, SPLIT_SAME, A);
   TcWeights wp = prep_weights(p + ".proj_out.weight", C, C, 1, "", 0);
   emit_tc(p + ".proj_out", A, TAPS_1X1, nullptr, wp, C, out, P(p + ".proj_out.bias", C), 0, x.p, x.ld);
 }
@@ -128,8 +123,7 @@ void UNetSimple::build_program() {
   // ---- scratch sizing ----
   size_t split_max = 0, hbuf_max = 0, att_tok = 0, att_c = 0, att_T = 0;
   int n_gn = 0;
-  std::vector<std::string> rb_names;
-  std::vector<int> rb_cout;
+  std::vector<EmbProj> projs;
   auto plan_conv_in = [&](int res, int Cin, bool up2) {
     split_max = std::max(split_max, (size_t)B_ * res * res * Cin * (up2 ? 4 : 1));
   };
@@ -138,8 +132,8 @@ void UNetSimple::build_program() {
     plan_conv_in(res, Cout, false);
     hbuf_max = std::max(hbuf_max, (size_t)B_ * res * res * Cout);
     n_gn += 2;
-    rb_names.push_back(p);
-    rb_cout.push_back(Cout);
+    // conv1.bias joins the projection bias: both are added to every pixel of conv1's output (models.py:119,121)
+    projs.push_back({p, p + ".temb_proj.weight", bias_sum(p + ".temb_proj.bias", p + ".conv1.bias", Cout), Cout});
   };
   auto plan_attn = [&](int res, int C) {
     plan_conv_in(res, C, false);
@@ -175,46 +169,8 @@ void UNetSimple::build_program() {
   alloc_common(split_max, hbuf_max);
   alloc_attention((size_t)B_ * att_tok * 3 * att_c, (size_t)B_ * att_T * att_T, (size_t)B_ * att_tok * att_c);
 
-  // ---- timestep embedding MLP + all per-block projections as one matrix (models.py:305-308, :121) ----
-  const int tch = c.ch * 4;
-  emb_ = (float*)arena_.alloc((size_t)B_ * c.ch * 4);
-  temb0_ = (float*)arena_.alloc((size_t)B_ * tch * 4);
-  temb_ = (float*)arena_.alloc((size_t)B_ * tch * 4);
-  freq_ = (float*)arena_.alloc((size_t)(c.ch / 2) * 4);
-  CUDA_CHECK(cudaMemcpy(freq_, P("__freq", c.ch / 2), (c.ch / 2) * 4, cudaMemcpyDeviceToDevice));
-  ca_total_ = 0;
-  for (size_t i = 0; i < rb_names.size(); ++i) {
-    ca_off_[rb_names[i]] = ca_total_;
-    ca_total_ += rb_cout[i];
-  }
-  tembW_all_ = (float*)arena_.alloc((size_t)ca_total_ * tch * 4);
-  tembB_all_ = (float*)arena_.alloc((size_t)ca_total_ * 4);
-  ca_all_ = (float*)arena_.alloc((size_t)B_ * ca_total_ * 4);
-  for (size_t i = 0; i < rb_names.size(); ++i) {
-    const std::string& p = rb_names[i];
-    const int off = ca_off_[p], co = rb_cout[i];
-    CUDA_CHECK(cudaMemcpy(tembW_all_ + (size_t)off * tch, P(p + ".temb_proj.weight", (long long)co * tch), (size_t)co * tch * 4,
-                          cudaMemcpyDeviceToDevice));
-    // conv1.bias joins the projection bias: both are added to every pixel of conv1's output (models.py:119,121)
-    const float* bs = bias_sum(p + ".temb_proj.bias", p + ".conv1.bias", co);
-    CUDA_CHECK(cudaMemcpy(tembB_all_ + off, bs, (size_t)co * 4, cudaMemcpyDeviceToDevice));
-  }
-
   // ---- program ----
-  {
-    float *t = t_in_, *emb = emb_, *t0 = temb0_, *t1 = temb_, *fr = freq_, *ca = ca_all_, *W = tembW_all_, *Bv = tembB_all_;
-    const float *w0 = P("temb.dense.0.weight", (long long)tch * c.ch), *b0 = P("temb.dense.0.bias", tch);
-    const float *w1 = P("temb.dense.1.weight", (long long)tch * tch), *b1 = P("temb.dense.1.bias", tch);
-    const int Bn = B_, chn = c.ch, cat = ca_total_;
-    add_op("temb", "temb", 0, 0, [=](cudaStream_t s) {
-      sinusoid(t, Bn, fr, chn, true, emb, s);
-      // temb = dense1(swish(dense0(emb))); every block consumes swish(temb) (models.py:121), so the activations are
-      // applied once at the producers' outputs
-      linear(emb, Bn, chn, w0, b0, tch, t0, tch, 0, 1, s);
-      linear(t0, Bn, tch, w1, b1, tch, t1, tch, 0, 1, s);
-      linear(t1, Bn, tch, W, Bv, cat, ca, cat, 0, 0, s);
-    });
-  }
+  emit_time_embed("temb", "temb.dense.0", "temb.dense.1", c.ch, true, nullptr, 0, projs);
   // concat buffers for the up path; hs[i] lives in cat[n_up-1-i].slice(Ch, Cs)
   std::vector<View> cat(n_up);
   for (int u = 0; u < n_up; ++u) cat[u] = new_view(upb[u].res, upb[u].res, upb[u].Ch + upb[u].Cs);
