@@ -120,6 +120,10 @@ _SIGS = {
     "ddnm_inverse_data_transform": (C.c_int, [_P, _LL, _I, _I, _P, _P]),
     "ddnm_finish_images": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
     "ddnm_conv_tc": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P]),
+    "ddnm_conv_tc_ex": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _I, _P, _I, _P, _P, _I, _P, _I, _I, _I, _I, C.POINTER(_D),
+                                  C.POINTER(_I), _P]),
+    "ddnm_gemm_tc": (C.c_int, [_P, _LL, _LL, _LL, _LL, _LL, _P, _LL, _LL, _LL, _LL, _LL, _I, _I, _I, _I, _I, _F, _P, _LL, _LL, _LL,
+                               _I, _P]),
     "ddnm_conv_direct": (C.c_int, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _I, _P, _P]),
     "ddnm_conv_stem_sr": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _I, _P, _I, C.POINTER(_F), _P]),
     "ddnm_conv_tc_bench": (C.c_int, [_I, _I, _I, _I, _I, _I, _I, C.POINTER(_F), C.POINTER(_D)]),

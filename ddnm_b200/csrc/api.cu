@@ -207,6 +207,20 @@ View mkview(float* p, int N, int H, int W, int C) {
   v.p = p; v.N = N; v.H = H; v.W = W; v.C = C; v.ld = C;
   return v;
 }
+// the SM count an engine built now would plan its launches for (ddnm_tc_debug_sm_count)
+int planned_sm_count() {
+  int dev = 0;
+  CUDA_CHECK(cudaGetDevice(&dev));
+  cudaDeviceProp prop;
+  CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
+  return engine_sm_count(prop);
+}
+// the fp16 product terms of the launches built while it lives (the launch builders read the global setting)
+struct TermsScope {
+  int prev;
+  explicit TermsScope(int t) : prev(tc_get_terms()) { tc_set_terms(t); }
+  ~TermsScope() { tc_set_terms(prev); }
+};
 }  // namespace
 
 extern "C" {
@@ -255,6 +269,104 @@ int ddnm_conv_tc(const float* x, int N, int H, int W, int Cin, const float* w, c
   if (side_x) split_conv_weight(side_w, Cout, CinSide, 1, wh, wl, ktot, taps * Cin, s);
   TcLaunch L = tc_make_launch(A, mode, side_x ? &S : nullptr, wh, wl, 1, Cout, ov, bias, 0, residual, Cout, 1.0f, sm_count());
   tc_run(L, s);
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  DDNM_API_END
+}
+
+int ddnm_conv_tc_ex(const float* x, int N, int H, int W, int Cin, const float* w, const float* chanadd, int ca_ld, int Cout, int mode,
+                    int up2, const float* side_x, int CinSide, const float* side_w, const float* residual, int res_mode, float* out,
+                    int out_ld, int split_k, int invariant, int terms, double* stats_out, int* split_used, void* stream) {
+  DDNM_API_BEGIN
+  DDNM_CHECK(x && w && out, "null argument");
+  DDNM_CHECK(mode >= TAPS_3X3 && mode <= TAPS_3X3_S2 && res_mode >= 0 && res_mode <= 2 && out_ld >= Cout && ca_ld >= 0,
+             "bad mode, res_mode, out_ld or ca_ld");
+  DDNM_CHECK(split_k == -1 || split_k == 1 || split_k == 2 || split_k == 4, "split_k must be -1 (the engine's rule), 1, 2 or 4");
+  cudaStream_t s = (cudaStream_t)stream;
+  Tmp tmp;
+  const TermsScope terms_scope(terms);
+  const int sms = planned_sm_count();
+  const int taps = mode == TAPS_1X1 ? 1 : 9;
+  int oH = H, oW = W;
+  int smode = SPLIT_SAME;
+  if (mode == TAPS_3X3_S2) { oH = H / 2; oW = W / 2; smode = SPLIT_S2D; DDNM_CHECK(!up2, "stride 2 with upsample"); }
+  if (up2) {
+    oH = 2 * H; oW = 2 * W;
+    // as UNetEngine::emit_up2_conv: a plain 3x3 on the upsampled map, never split
+    DDNM_CHECK(mode == TAPS_3X3 && !side_x && !residual && split_k <= 1, "upsample path: plain unsplit 3x3 only");
+  }
+  const size_t pe = (size_t)N * H * W * Cin;
+  SplitView A;
+  A.hi = tmp.get<__half>(pe); A.lo = tmp.get<__half>(pe); A.C = Cin;
+  if (smode == SPLIT_S2D) { A.N = 4 * N; A.H = oH; A.W = oW; } else { A.N = N; A.H = H; A.W = W; }
+  gn_apply_split(mkview(const_cast<float*>(x), N, H, W, Cin), 1, false, nullptr, nullptr, 0.f, false, smode, A.hi, A.lo, s);
+  View ov = mkview(out, N, oH, oW, Cout);
+  ov.ld = out_ld;
+  if (stats_out) {
+    ov.st = tmp.get<StatAcc>((size_t)N * Cout * 2);
+    ov.st_ld = Cout;
+    CUDA_CHECK(cudaMemsetAsync(ov.st, 0, (size_t)N * Cout * 2 * sizeof(StatAcc), s));
+  }
+  int S = 1;
+  if (up2) {
+    // the four parity phases add into one stats buffer, as in UNetEngine::emit_up2_conv
+    const size_t per_phase = (size_t)Cout * 4 * Cin;
+    __half* wh = tmp.get<__half>(4 * per_phase);
+    __half* wl = tmp.get<__half>(4 * per_phase);
+    presum_up2_weights(w, Cout, Cin, wh, wl, s);
+    for (int ph = 0; ph < 4; ++ph)
+      tc_run(tc_make_up2_launch(A, wh + ph * per_phase, wl + ph * per_phase, Cout, ov, chanadd, ca_ld, ph >> 1, ph & 1, sms, invariant != 0), s);
+  } else {
+    SplitView Sv;
+    if (side_x) {
+      const size_t se = (size_t)N * oH * oW * CinSide;
+      Sv.hi = tmp.get<__half>(se); Sv.lo = tmp.get<__half>(se); Sv.N = N; Sv.H = oH; Sv.W = oW; Sv.C = CinSide;
+      gn_apply_split(mkview(const_cast<float*>(side_x), N, oH, oW, CinSide), 1, false, nullptr, nullptr, 0.f, false, SPLIT_SAME,
+                     Sv.hi, Sv.lo, s);
+    }
+    const int ktot = taps * Cin + (side_x ? CinSide : 0);
+    __half* wh = tmp.get<__half>((size_t)Cout * ktot);
+    __half* wl = tmp.get<__half>((size_t)Cout * ktot);
+    split_conv_weight(w, Cout, Cin, taps, wh, wl, ktot, 0, s);
+    if (side_x) split_conv_weight(side_w, Cout, CinSide, 1, wh, wl, ktot, taps * Cin, s);
+    TcConvPlan P = tc_plan_conv(A, mode, side_x ? &Sv : nullptr, wh, wl, Cout, ov, chanadd, ca_ld, residual, Cout, res_mode, sms,
+                                invariant != 0, split_k);
+    if (P.S > 1) tc_set_partials(P, tmp.get<float>((size_t)P.part_elems));
+    tc_run_conv(P, s);
+    S = P.S;
+  }
+  CUDA_CHECK(cudaStreamSynchronize(s));
+  if (split_used) *split_used = S;
+  if (stats_out) {
+    std::vector<StatAcc> h((size_t)N * Cout * 2);
+    CUDA_CHECK(cudaMemcpy(h.data(), ov.st, h.size() * sizeof(StatAcc), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < h.size(); ++i) stats_out[i] = stat_value(h[i]);
+  }
+  DDNM_API_END
+}
+
+int ddnm_gemm_tc(const float* a, long long a_numel, long long a_off, long long a_s_row, long long a_s_head, long long a_s_img,
+                 const float* b, long long b_numel, long long b_off, long long b_s_row, long long b_s_head, long long b_s_img, int M,
+                 int N, int K, int heads, int images, float alpha, float* out, long long out_sn, long long out_sy, long long out_sx,
+                 int invariant, void* stream) {
+  DDNM_API_BEGIN
+  DDNM_CHECK(a && b && out && M > 0 && N > 0 && K > 0 && heads > 0 && images > 0, "null or empty argument");
+  cudaStream_t s = (cudaStream_t)stream;
+  Tmp tmp;
+  auto operand = [&](const float* src, long long numel, long long off, long long rows, long long s_row, long long s_head,
+                     long long s_img) {
+    DDNM_CHECK(numel % 8 == 0 && off >= 0 && s_row > 0 && s_head > 0 && s_img > 0, "GEMM operand: bad size or strides");
+    DDNM_CHECK(off + (K - 1) + (rows - 1) * s_row + (heads - 1) * s_head + (images - 1) * s_img < numel,
+               "GEMM operand reaches past its buffer");
+    __half* hi = tmp.get<__half>((size_t)numel);
+    __half* lo = tmp.get<__half>((size_t)numel);
+    // the attention core's raw split (elementwise), the buffer viewed as rows of 8 channels
+    gn_apply_split(mkview(const_cast<float*>(src), 1, 1, (int)(numel / 8), 8), 1, false, nullptr, nullptr, 0.f, false, SPLIT_SAME,
+                   hi, lo, s);
+    return GemmOperand{hi + off, lo + off, s_row, s_head, s_img};
+  };
+  const GemmOperand A = operand(a, a_numel, a_off, M, a_s_row, a_s_head, a_s_img);
+  const GemmOperand B = operand(b, b_numel, b_off, N, b_s_row, b_s_head, b_s_img);
+  tc_run(tc_make_gemm_launch(A, B, M, N, K, heads, images, out, out_sn, out_sy, out_sx, alpha, planned_sm_count(), invariant != 0), s);
   CUDA_CHECK(cudaStreamSynchronize(s));
   DDNM_API_END
 }

@@ -299,7 +299,7 @@ __device__ __forceinline__ void two_sum_acc(float& sum, float& comp, float v) {
   comp = __fadd_rn(comp, __fadd_rn(__fadd_rn(sum, -__fadd_rn(s, -bb)), __fadd_rn(v, -bb)));
   sum = s;
 }
-__device__ __forceinline__ double stat_value(const StatAcc& a) {
+__host__ __device__ __forceinline__ double stat_value(const StatAcc& a) {
   return ((double)a.hi * 4294967296.0 + (double)a.lo) * (1.0 / 281474976710656.0);
 }
 

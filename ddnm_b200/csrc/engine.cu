@@ -32,6 +32,9 @@ void engine_debug_sm_count(int n) {
   DDNM_CHECK(n >= 0, "SM count must be 0 (the device's) or positive");
   g_sm_count = n;
 }
+int engine_sm_count(const cudaDeviceProp& prop) {
+  return g_sm_count > 0 ? std::min(g_sm_count, prop.multiProcessorCount) : prop.multiProcessorCount;
+}
 
 UNetEngine::UNetEngine(int batch, int in_channels, int out_ch, int resolution, int groups, float eps)
     : B_(batch), in_ch_(in_channels), out_ch_(out_ch), R_(resolution), groups_(groups), eps_(eps) {
@@ -41,7 +44,7 @@ UNetEngine::UNetEngine(int batch, int in_channels, int out_ch, int resolution, i
   cudaDeviceProp prop;
   CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
   DDNM_CHECK(prop.major == 9 && prop.minor == 0, "ddnm_b200 kernels are built for sm_90a (H100) only");
-  num_sms_ = g_sm_count > 0 ? std::min(g_sm_count, prop.multiProcessorCount) : prop.multiProcessorCount;
+  num_sms_ = engine_sm_count(prop);
 }
 
 UNetEngine::~UNetEngine() {
@@ -165,33 +168,15 @@ void UNetEngine::emit_gn_split(const std::string& name, const View& x, const std
 
 void UNetEngine::emit_tc(const std::string& name, const SplitView& a, int mode, const SplitView* side, const TcWeights& w,
                          int Cout, const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int res_mode) {
-  TcLaunch L = tc_make_launch(a, mode, side, w.hi, w.lo, 1, Cout, out, chanadd, ca_ld, residual, ldr, 1.0f, num_sms_, res_mode, invariant_);
+  TcConvPlan P = tc_plan_conv(a, mode, side, w.hi, w.lo, Cout, out, chanadd, ca_ld, residual, ldr, res_mode, num_sms_, invariant_);
+  const TcLaunch& L = P.L;
   const double bytes = (double)a.N * a.H * a.W * a.C * 4 + (side ? (double)side->N * side->H * side->W * side->C * 4 : 0) +
                        (double)Cout * w.ktot * 4 + (double)out.pixels() * Cout * 4 * (residual ? 2 : 1);
-  // split-K: few tiles walking a long K one k-block after the other (the 8x8 level: 32-64 CTAs, 72-144 k-blocks) are latency-bound;
-  // 2 or 4 CTAs per tile, each over its own k-block range into its own partial buffer, then one small deterministic reduce
-  const int tiles = L.p.tiles_x * L.p.tiles_y * L.p.tiles_n * L.p.n_tiles, kblocks = L.p.kb0 + L.p.kb1;
-  static const bool split_on = std::getenv("DDNM_SPLITK") == nullptr || std::atoi(std::getenv("DDNM_SPLITK")) != 0;
-  int S = 1;
-  if (split_on && res_mode == 0 && kblocks >= 32) {
-    // batch-invariant mode: S is part of an element's arithmetic (the k-block ranges and their fixed-order sum), so it follows the
-    // per-image shape alone — 2 on the maps of at most 64 pixels, the 8x8 level where B = 16 splits by the tile count as well
-    if (invariant_) S = out.H * out.W <= 64 ? 2 : 1;
-    else if (2 * tiles <= num_sms_) S = 4 * tiles <= num_sms_ ? 4 : 2;
-  }
-  if (S > 1) {
-    const long long stride = out.pixels() * Cout;
-    float* part = (float*)arena_.alloc((size_t)S * stride * sizeof(float));
-    const View pv = view_of(part, out.H, out.W, Cout);
-    TcLaunch Ls = tc_make_launch(a, mode, side, w.hi, w.lo, 1, Cout, pv, nullptr, 0, nullptr, 0, 1.0f, num_sms_, 0, invariant_);
-    DDNM_CHECK(Ls.BN == L.BN, "split-K: tile shape changed");
-    Ls.p.split_k = S;
-    Ls.p.split_stride = stride;
-    Ls.halo = false;   // k-block ranges of a split need not be whole A units
-    Ls.grid = std::min(tiles * S, num_sms_);
-    add_op(name, "tc", L.flops, bytes, [Ls](cudaStream_t s) { tc_run(Ls, s); });
-    add_op(name + ".splitk_reduce", "reduce", 0, (double)(S + 1 + (residual ? 1 : 0)) * stride * 4,
-           [=](cudaStream_t s) { splitk_reduce(part, S, stride, out, chanadd, ca_ld, residual, ldr, s); });
+  if (P.S > 1) {
+    tc_set_partials(P, (float*)arena_.alloc((size_t)P.part_elems * sizeof(float)));
+    add_op(name, "tc", L.flops, bytes, [L](cudaStream_t s) { tc_run(L, s); });
+    add_op(name + ".splitk_reduce", "reduce", 0, (double)(P.S + 1 + (residual ? 1 : 0)) * (P.part_elems / P.S) * 4,
+           [P](cudaStream_t s) { tc_run_split_reduce(P, s); });
     return;
   }
   add_op(name, "tc", L.flops, bytes, [L](cudaStream_t s) { tc_run(L, s); });

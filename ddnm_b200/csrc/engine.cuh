@@ -62,6 +62,7 @@ struct OpenAICfg {
 
 // tests: engines built after the call size their grids and launch policy for min(n, the device's count) SMs (0 = the device's count)
 void engine_debug_sm_count(int n);
+int engine_sm_count(const cudaDeviceProp& prop);   // the SM count launches are planned for on that device
 
 class UNetEngine {
  public:

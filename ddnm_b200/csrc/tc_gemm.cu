@@ -36,6 +36,8 @@
 
 #include <cstdlib>
 
+#include "kernels.cuh"
+
 namespace ddnm {
 
 static constexpr int BM = 128;
@@ -981,6 +983,60 @@ TcLaunch tc_make_up2_launch(const SplitView& src, const __half* w_hi, const __ha
   p.out_sy = 2LL * out.W * out.ld;
   p.out_sn = (long long)out.H * out.W * out.ld;
   return L;
+}
+
+TcConvPlan tc_plan_conv(const SplitView& src0, int mode0, const SplitView* src1, const __half* w_hi, const __half* w_lo, int Cout,
+                        const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int res_mode, int num_sms,
+                        bool invariant, int split_k) {
+  TcConvPlan P;
+  P.out = out; P.chanadd = chanadd; P.ca_ld = ca_ld; P.residual = residual; P.ldr = ldr;
+  P.L = tc_make_launch(src0, mode0, src1, w_hi, w_lo, 1, Cout, out, chanadd, ca_ld, residual, ldr, 1.0f, num_sms, res_mode, invariant);
+  // split-K: few tiles walking a long K one k-block after the other (the 8x8 level: 32-64 CTAs, 72-144 k-blocks) are latency-bound;
+  // 2 or 4 CTAs per tile, each over its own k-block range into its own partial buffer, then one small deterministic reduce
+  const TcParams& p = P.L.p;
+  const int tiles = p.tiles_x * p.tiles_y * p.tiles_n * p.n_tiles, kblocks = p.kb0 + p.kb1;
+  static const bool split_on = std::getenv("DDNM_SPLITK") == nullptr || std::atoi(std::getenv("DDNM_SPLITK")) != 0;
+  int S = 1;
+  if (split_k > 0) {
+    DDNM_CHECK(split_k == 1 || split_k == 2 || split_k == 4, "split_k must be 1, 2 or 4");
+    DDNM_CHECK(split_k == 1 || (res_mode == 0 && kblocks >= split_k), "split-K needs res_mode 0 and a k-block per split");
+    S = split_k;
+  } else if (split_on && res_mode == 0 && kblocks >= 32) {
+    // batch-invariant mode: S is part of an element's arithmetic (the k-block ranges and their fixed-order sum), so it follows the
+    // per-image shape alone — 2 on the maps of at most 64 pixels, the 8x8 level where B = 16 splits by the tile count as well
+    if (invariant) S = out.H * out.W <= 64 ? 2 : 1;
+    else if (2 * tiles <= num_sms) S = 4 * tiles <= num_sms ? 4 : 2;
+  }
+  if (S == 1) return P;
+  P.S = S;
+  const long long stride = out.pixels() * Cout;
+  P.part_elems = S * stride;
+  View pv = out;   // the partial buffers: dense [pixels][Cout], no epilogue terms, no GroupNorm sums (the reduce does those)
+  pv.p = nullptr; pv.ld = Cout; pv.st = nullptr; pv.st_ld = 0;
+  TcLaunch Ls = tc_make_launch(src0, mode0, src1, w_hi, w_lo, 1, Cout, pv, nullptr, 0, nullptr, 0, 1.0f, num_sms, 0, invariant);
+  DDNM_CHECK(Ls.BN == P.L.BN, "split-K: tile shape changed");
+  Ls.p.split_k = S;
+  Ls.p.split_stride = stride;
+  Ls.halo = false;   // k-block ranges of a split need not be whole A units
+  Ls.grid = std::min(tiles * S, num_sms);
+  P.L = Ls;
+  return P;
+}
+
+void tc_set_partials(TcConvPlan& P, float* part) {
+  DDNM_CHECK(P.S > 1 && part != nullptr, "partial buffer for an unsplit plan");
+  P.part = part;
+  P.L.p.out = part;
+}
+
+void tc_run_split_reduce(const TcConvPlan& P, cudaStream_t stream) {
+  DDNM_CHECK(P.S > 1 && P.part != nullptr, "split-K reduce without partial buffers");
+  splitk_reduce(P.part, P.S, P.part_elems / P.S, P.out, P.chanadd, P.ca_ld, P.residual, P.ldr, stream);
+}
+
+void tc_run_conv(const TcConvPlan& P, cudaStream_t stream) {
+  tc_run(P.L, stream);
+  if (P.S > 1) tc_run_split_reduce(P, stream);
 }
 
 TcLaunch tc_make_gemm_launch(const GemmOperand& A, const GemmOperand& B, int M, int N, int K, int heads, int images, float* out,

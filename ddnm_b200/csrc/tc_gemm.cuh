@@ -71,6 +71,28 @@ void tc_run(const TcLaunch& L, cudaStream_t stream);
 TcLaunch tc_make_up2_launch(const SplitView& src, const __half* w_hi, const __half* w_lo, int Cout, const View& out, const float* chanadd,
                             int ca_ld, int py, int px, int num_sms, bool invariant = false);
 
+// A convolution as it runs: one launch, or (S > 1, split-K) S CTAs per tile over disjoint k-block ranges into S partial buffers,
+// then splitk_reduce (fixed-order sum + chanadd + residual + GroupNorm sums of `out`).
+struct TcConvPlan {
+  TcLaunch L;                   // S > 1: the partial launch, writing to `part` (see tc_set_partials)
+  int S = 1;
+  long long part_elems = 0;     // S > 1: floats of the partial buffer (S * pixels * Cout)
+  float* part = nullptr;
+  View out;
+  const float* chanadd = nullptr;
+  int ca_ld = 0;
+  const float* residual = nullptr;
+  int ldr = 0;
+};
+// The engine's convolution: tc_make_launch, and split-K where few tiles walk a long K (the 8x8 level).  split_k < 0: that rule
+// (env DDNM_SPLITK=0 turns it off); 1, 2, 4: forced (res_mode 0 only).  A split plan needs tc_set_partials before it runs.
+TcConvPlan tc_plan_conv(const SplitView& src0, int mode0, const SplitView* src1, const __half* w_hi, const __half* w_lo, int Cout,
+                        const View& out, const float* chanadd, int ca_ld, const float* residual, int ldr, int res_mode, int num_sms,
+                        bool invariant, int split_k = -1);
+void tc_set_partials(TcConvPlan& plan, float* part);   // part: plan.part_elems floats
+void tc_run_split_reduce(const TcConvPlan& plan, cudaStream_t stream);   // S > 1: the second launch of the plan
+void tc_run_conv(const TcConvPlan& plan, cudaStream_t stream);           // the whole plan
+
 // Strided fp16 (hi, lo) operand for the batched-GEMM builder: element (k, row, head, image) at
 // base[k + row*s_row + head*s_head + image*s_img]; k extent = K (multiple of 8; base and strides 16-byte aligned).
 struct GemmOperand {

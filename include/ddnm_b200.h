@@ -307,6 +307,23 @@ int ddnm_finish_images(const float* x, const float* orig, int B, int C, int H, i
  * ---------------------------------------------------------------------------------------------- */
 int ddnm_conv_tc(const float* x, int N, int H, int W, int Cin, const float* w, const float* bias, int Cout, int mode, int up2,
                  const float* side_x, int CinSide, const float* side_w, const float* residual, float* out, void* stream);
+/* ddnm_conv_tc with every epilogue feature of the engine's convolutions, built by the engine's launch builders (tests):
+ * chanadd [rows][ca_ld] is added per (image, channel) (ca_ld = 0: one row for every image); residual (NHWC, Cout channels) is added
+ * at res_mode 0: the same pixel, 1: nearest x2 of an oH/2 x oW/2 map, 2: the 2x2 average of a 2oH x 2oW map; out has row stride
+ * out_ld >= Cout; split_k: -1 the engine's split-K rule, 1 / 2 / 4 forced; invariant: batch-invariant launches; terms: 3 (fp32-grade)
+ * or 1 (fast fp16).  stats_out (optional, host) receives the GroupNorm sums of the output, [N][Cout][2] {sum, sum of squares};
+ * split_used (optional) the split-K factor the launch ran with.  up2: the four parity-phase launches, unsplit, chanadd only. */
+int ddnm_conv_tc_ex(const float* x, int N, int H, int W, int Cin, const float* w, const float* chanadd, int ca_ld, int Cout, int mode,
+                    int up2, const float* side_x, int CinSide, const float* side_w, const float* residual, int res_mode, float* out,
+                    int out_ld, int split_k, int invariant, int terms, double* stats_out, int* split_used, void* stream);
+/* the attention GEMM (tests): out[img*out_sn + head*out_sy + m*out_sx + n] = alpha * sum_k A[k, m, head, img] * B[k, n, head, img]
+ * with A[k, m, head, img] = a[a_off + k + m*a_s_row + head*a_s_head + img*a_s_img] (B likewise over n); a and b (fp32, a_numel and
+ * b_numel elements, multiples of 8) are split to fp16 (hi, lo) as the attention core splits qkv.  M % 128 == 0, N % 8 == 0,
+ * K % 8 == 0; offsets and strides multiples of 8. */
+int ddnm_gemm_tc(const float* a, long long a_numel, long long a_off, long long a_s_row, long long a_s_head, long long a_s_img,
+                 const float* b, long long b_numel, long long b_off, long long b_s_row, long long b_s_head, long long b_s_img, int M,
+                 int N, int K, int heads, int images, float alpha, float* out, long long out_sn, long long out_sy, long long out_sx,
+                 int invariant, void* stream);
 int ddnm_conv_direct(const float* x, int N, int H, int W, int Cin, const float* w, const float* bias, int Cout, int mode, int up2,
                      float* out, void* stream);
 /* the super-resolution stem (SuperResModel's input_blocks.0): out NHWC [N,H,W,Cout] = conv3x3(cat([x, bilinear(low_res)])) + bias

@@ -1,9 +1,10 @@
 """Ping-pong form of the wgmma convolution: two consumer warpgroups that each own a whole 128-row tile and take turns on the tensor
 cores, so one tile's epilogue overlaps the next tile's MMAs.  It issues the products of the three-instruction form in the same order
 for every output element, so a convolution is bit-identical to conv_tc_kernel with DUAL off.  Every op-level case has more tiles than
-CTAs, so the launch runs on the ping-pong kernel; with DUAL on (the default) the other kernel would not give the same bits.  The
-engine-level checks cover what the op-level entry does not reach (split-K, residual modes 1 / 2, attention GEMMs, GroupNorm sums,
-one-product fp16 mode): ping-pong on and off agree to fp32 rounding of the statistics, and each is bit-reproducible."""
+CTAs, so the launch runs on the ping-pong kernel; with DUAL on (the default) the other kernel would not give the same bits.  Split-K,
+residual modes 1 / 2, per-image channel adds, GroupNorm sums, attention GEMMs and the one-product fp16 mode are checked op by op
+against fp64 in test_gpu_epilogue.py; the engine-level checks here add that whole forwards with ping-pong on and off agree to fp32
+rounding of the statistics, and that each is bit-reproducible."""
 import pytest
 import torch
 

@@ -79,6 +79,37 @@ def test_library_loads_and_exports_every_declared_symbol():
     assert _lib.lib().ddnm_version() >= 100
 
 
+def _ctype_of(decl):
+    """ctypes type the binding should use for one C parameter declaration of the header"""
+    t = re.sub(r"\bconst\b", "", decl).strip()
+    t = re.sub(r"\s+\w+$", "", t) if not t.endswith("*") else t   # drop the parameter name
+    t = re.sub(r"\s+", " ", t).replace(" *", "*").strip()
+    scalar = {"int": ctypes.c_int, "long long": ctypes.c_longlong, "float": ctypes.c_float, "double": ctypes.c_double,
+              "unsigned": ctypes.c_uint, "void*": ctypes.c_void_p, "char*": ctypes.c_char_p}
+    if t in scalar:
+        return scalar[t]
+    if t in ("double*", "int*", "long long*", "float*"):
+        return ("ptr", t[:-1])   # an out-parameter the binding types, or a device buffer passed as void*
+    return None
+
+
+def test_new_op_entry_signatures_match_the_header():
+    """the ctypes argument lists of the op-level test entries agree with their prototypes, parameter by parameter"""
+    from ddnm_b200 import _lib
+    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "ddnm_b200.h")).read(), flags=re.S)
+    for name in ("ddnm_conv_tc_ex", "ddnm_gemm_tc", "ddnm_conv_tc"):
+        params = re.search(name + r"\s*\(([^)]*)\)", hdr).group(1).split(",")
+        res, args = _lib._SIGS[name]
+        assert res is ctypes.c_int and len(args) == len(params), name
+        for decl, got in zip(params, args):
+            want = _ctype_of(decl)
+            if isinstance(want, tuple):
+                base = {"double": ctypes.c_double, "int": ctypes.c_int, "long long": ctypes.c_longlong, "float": ctypes.c_float}[want[1]]
+                assert got in (ctypes.c_void_p, ctypes.POINTER(base)), f"{name}: {decl.strip()} bound as {got}"
+            else:
+                assert want is not None and got is want, f"{name}: {decl.strip()} bound as {got}"
+
+
 def test_fails_loudly_without_gpu_or_library(monkeypatch, tmp_path):
     from ddnm_b200 import _lib
     from ddnm_b200.model import Model
