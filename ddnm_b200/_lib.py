@@ -46,7 +46,7 @@ class OperatorDesc(C.Structure):
 
 class SimpleDeg(C.Structure):
     _fields_ = [("use_mask", C.c_int), ("use_gray", C.c_int), ("scale", C.c_int), ("img_dim", C.c_int), ("channels", C.c_int),
-                ("mask", C.c_void_p)]
+                ("mask", C.c_void_p), ("image_mask", C.c_void_p)]
 
 
 class HqScalars(C.Structure):
@@ -116,6 +116,7 @@ _SIGS = {
     "ddnm_hq_canvas": (C.c_int, [_P, _I, _I, _I, _I, _I, _P, _P]),
     "ddnm_hq_step": (C.c_int, [C.POINTER(SimpleDeg), _P, _P, _I, _P, _P, _I, _I, _P, _P, _P, C.POINTER(HqScalars), _I, _P, _P, _P, _P]),
     "ddnm_hq_undo": (C.c_int, [_P, _P, _F, _F, _LL, _P]),
+    "ddnm_hq_canvas_masked": (C.c_int, [C.POINTER(SimpleDeg), _P, _I, _P, _P, _P]),
     "ddnm_data_transform": (C.c_int, [_P, _LL, _P, _P, _I, _I, _P, _P]),
     "ddnm_inverse_data_transform": (C.c_int, [_P, _LL, _I, _I, _P, _P]),
     "ddnm_finish_images": (C.c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P]),

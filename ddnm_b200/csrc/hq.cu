@@ -5,6 +5,7 @@
 // plus the canvas preparation Ap(A_temp(gt)) of :651-655 for an arbitrary H x W.  The window / time loops stay on the host
 // (ddnm_b200/hq.py), as in the reference; every tensor operation of a step runs here.
 #include <cmath>
+#include <type_traits>
 
 #include "../../include/ddnm_b200.h"
 #include "api_util.cuh"
@@ -29,6 +30,17 @@ __global__ void hq_x0_kernel(const float* __restrict__ x, const float* __restric
 
 struct HqRect { int dy, dx, h, w, sy, sx; };   // x0_hat[:, :, dy:dy+h, dx:dx+w] = canvas[:, :, sy:sy+h, sx:sx+w]
 
+// the mask-shift overwrite of x0_hat element (bc, py, px); the second rectangle is applied after the first (reference order
+// :363-384), so it wins where they overlap
+__device__ __forceinline__ float hq_shift(float v, const float* __restrict__ canvas, int cH, int cW, const HqRect& r0, const HqRect& r1,
+                                          long long bc, int py, int px) {
+  if (r0.h > 0 && py >= r0.dy && py < r0.dy + r0.h && px >= r0.dx && px < r0.dx + r0.w)
+    v = canvas[(bc * cH + (r0.sy + py - r0.dy)) * cW + (r0.sx + px - r0.dx)];
+  if (r1.h > 0 && py >= r1.dy && py < r1.dy + r1.h && px >= r1.dx && px < r1.dx + r1.w)
+    v = canvas[(bc * cH + (r1.sy + py - r1.dy)) * cW + (r1.sx + px - r1.dx)];
+  return v;
+}
+
 // x0_hat = lambda*Apy + x0_t - lambda*ApA; mask-shift overwrite; mean = coef1*x0_hat + coef2*x (+ gamma*grad);
 // x_next = mean + nonzero*sqrt(gamma)*noise
 // GEN: the draw is generated in registers from gen, z unused
@@ -42,11 +54,7 @@ __global__ void hq_combine_kernel(const float* __restrict__ x, const float* __re
   const int px = (int)(i % D), py = (int)((i / D) % D);
   const long long bc = i / ((long long)D * D);
   float v = __fsub_rn(__fadd_rn(__fmul_rn(s.lambda_t, apy[i]), x0t[i]), __fmul_rn(s.lambda_t, apa[i]));
-  // the second rectangle is applied after the first (reference order :363-384), so it wins where they overlap
-  if (r0.h > 0 && py >= r0.dy && py < r0.dy + r0.h && px >= r0.dx && px < r0.dx + r0.w)
-    v = canvas[(bc * cH + (r0.sy + py - r0.dy)) * cW + (r0.sx + px - r0.dx)];
-  if (r1.h > 0 && py >= r1.dy && py < r1.dy + r1.h && px >= r1.dx && px < r1.dx + r1.w)
-    v = canvas[(bc * cH + (r1.sy + py - r1.dy)) * cW + (r1.sx + px - r1.dx)];
+  v = hq_shift(v, canvas, cH, cW, r0, r1, bc, py, px);
   x0hat[i] = v;
   float mean = __fadd_rn(__fmul_rn(s.coef1, v), __fmul_rn(s.coef2, x[i]));
   if (grad) mean = __fadd_rn(mean, __fmul_rn(s.gamma_t, grad[i]));
@@ -58,6 +66,95 @@ __global__ void hq_combine_kernel(const float* __restrict__ x, const float* __re
     zi = z[i];
   }
   xn[i] = __fadd_rn(mean, __fmul_rn(__fmul_rn(s.nonzero, sqrtf(s.gamma_t)), zi));
+}
+
+// ---- per-image keep mask (hq_demo face256, :601-622): A(z) = pool_S(gray(z*m)), Ap(v) = gray2color(MeanUpsample_S(v))*m, with m
+// the (B,3,D,D) gt_keep_mask, multiplied (not selected: PNG edge pixels are fractional).  inpainting is S = 1 without gray, so
+// Ap(A(z)) = z*m*m needs no pooling; otherwise one pass pools A into y [B, G, D/S, D/S] (G = 1 with gray, else 3).
+struct HqMask {
+  const float* m;   // [B,3,D,D]
+  int gray, S, D;
+};
+
+__device__ __forceinline__ float hq_x0_at(const float* __restrict__ x, const float* __restrict__ mo, long long mo_stride, float c_recip,
+                                          float c_recipm1, int clip, long long b, long long r, long long img) {
+  float v = __fsub_rn(__fmul_rn(c_recip, x[b * img + r]), __fmul_rn(c_recipm1, mo[b * mo_stride + r]));
+  if (clip) v = fminf(fmaxf(v, -1.0f), 1.0f);
+  return v;
+}
+
+// y[b, g, py, px] = A(z) of one S x S patch; z = x0_t from (x, eps) (X0) or `in` itself (the canvas's gt).  Pixels are summed in
+// row-major order and divided once, as the simplified operators do.
+template <bool X0>
+__global__ void hq_mask_A_kernel(const float* __restrict__ in, const float* __restrict__ mo, long long mo_stride, ddnm_hq_scalars s,
+                                 HqMask q, float* __restrict__ y, int B) {
+  const int S = q.S, D = q.D, yd = D / S, G = q.gray ? 1 : 3;
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= (long long)B * G * yd * yd) return;
+  const int px = (int)(g % yd), py = (int)((g / yd) % yd), ch = (int)((g / ((long long)yd * yd)) % G);
+  const long long b = g / ((long long)G * yd * yd), HW = (long long)D * D, img = 3 * HW;
+  const float cf = (float)(1.0 / 3.0);
+  auto z = [&](int c, long long o) {
+    const long long r = c * HW + o;
+    const float v = X0 ? hq_x0_at(in, mo, mo_stride, s.c_recip, s.c_recipm1, s.clip, b, r, img) : in[b * img + r];
+    return __fmul_rn(v, q.m[b * img + r]);
+  };
+  float acc = 0.f;
+  for (int k = 0; k < S * S; ++k) {
+    const long long o = (long long)(py * S + k / S) * D + (px * S + k % S);
+    const float t = q.gray ? __fadd_rn(__fadd_rn(__fmul_rn(z(0, o), cf), __fmul_rn(z(1, o), cf)), __fmul_rn(z(2, o), cf)) : z(ch, o);
+    acc = __fadd_rn(acc, t);
+  }
+  y[g] = S > 1 ? __fdiv_rn(acc, (float)(S * S)) : acc;
+}
+
+// Ap(A(z)) at element (b, c, py, px) = flat index i, z_i = that element of z
+template <bool POOL>
+__device__ __forceinline__ float hq_mask_ApA(const HqMask& q, const float* __restrict__ y, float zi, long long i, long long b, int c,
+                                             int py, int px) {
+  const float m = q.m[i];
+  if (!POOL) return __fmul_rn(__fmul_rn(zi, m), m);
+  const int yd = q.D / q.S;
+  float w = y[((b * (q.gray ? 1 : 3) + (q.gray ? 0 : c)) * yd + py / q.S) * yd + px / q.S];
+  if (q.gray) {
+    const float cf = (float)(1.0 / 3.0);
+    const float basef = (float)((1.0 / 3.0) * (1.0 / 3.0) + (1.0 / 3.0) * (1.0 / 3.0) + (1.0 / 3.0) * (1.0 / 3.0));
+    w = __fdiv_rn(__fmul_rn(w, cf), basef);
+  }
+  return __fmul_rn(w, m);
+}
+
+// the whole step of hq_combine_kernel with x0_t and Ap(A(x0_t)) computed in place (y: the pooled A(x0_t) when POOL)
+template <bool POOL, bool GEN>
+__global__ void hq_mask_step_kernel(const float* __restrict__ x, const float* __restrict__ mo, long long mo_stride, HqMask q,
+                                    const float* __restrict__ y, const float* __restrict__ apy, const float* __restrict__ canvas, int cH,
+                                    int cW, HqRect r0, HqRect r1, const float* __restrict__ grad, const float* __restrict__ z,
+                                    ddnm_hq_scalars s, float* __restrict__ x0hat, float* __restrict__ xn, long long n, NoiseSrc gen) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int D = q.D;
+  const long long HW = (long long)D * D, img = 3 * HW, b = i / img, r = i - b * img, bc = i / HW;
+  const int c = (int)(r / HW), py = (int)((r / D) % D), px = (int)(r % D);
+  const float x0 = hq_x0_at(x, mo, mo_stride, s.c_recip, s.c_recipm1, s.clip, b, r, img);
+  const float apa = hq_mask_ApA<POOL>(q, y, x0, i, b, c, py, px);
+  float v = __fsub_rn(__fadd_rn(__fmul_rn(s.lambda_t, apy[i]), x0), __fmul_rn(s.lambda_t, apa));
+  v = hq_shift(v, canvas, cH, cW, r0, r1, bc, py, px);
+  x0hat[i] = v;
+  float mean = __fadd_rn(__fmul_rn(s.coef1, v), __fmul_rn(s.coef2, x[i]));
+  if (grad) mean = __fadd_rn(mean, __fmul_rn(s.gamma_t, grad[i]));
+  const float zi = GEN ? noise_at(gen, (int)b, r) : z[i];
+  xn[i] = __fadd_rn(mean, __fmul_rn(__fmul_rn(s.nonzero, sqrtf(s.gamma_t)), zi));
+}
+
+// canvas of a masked degradation: apy = Ap(A(gt))
+template <bool POOL>
+__global__ void hq_mask_canvas_kernel(const float* __restrict__ gt, HqMask q, const float* __restrict__ y, float* __restrict__ apy,
+                                      long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int D = q.D;
+  const long long HW = (long long)D * D, b = i / (3 * HW), r = i - b * 3 * HW;
+  apy[i] = hq_mask_ApA<POOL>(q, y, gt[i], i, b, (int)(r / HW), (int)((r / D) % D), (int)(r % D));
 }
 
 // x = sqrt(1 - beta)*x + sqrt(beta)*noise            (:211-217)
@@ -103,6 +200,12 @@ __global__ void hq_canvas_kernel(const float* __restrict__ gt, float* __restrict
 }  // namespace ddnm
 
 using namespace ddnm;
+static HqMask hq_mask(const ddnm_simple_deg* d) {
+  DDNM_CHECK(d->channels == 3 && !d->use_mask && d->scale >= 1 && d->img_dim > 0 && d->img_dim % d->scale == 0,
+             "per-image mask: 3 channels, no shared mask plane, a scale dividing the image size");
+  return HqMask{d->image_mask, d->use_gray ? 1 : 0, d->scale, d->img_dim};
+}
+
 // one mask-shift step with the draw from a tape or generated (ddnm_hq_step / ddnm_hq_step_seeded)
 static void hq_step(const ddnm_simple_deg* deg, const float* x, const float* model_out, int out_ch, const float* apy, const float* canvas,
                     int canvas_h, int canvas_w, const int* rects, const float* grad, const NoiseSrc& noise, const ddnm_hq_scalars* sc,
@@ -111,16 +214,39 @@ static void hq_step(const ddnm_simple_deg* deg, const float* x, const float* mod
   DDNM_CHECK(deg->channels == 3 && (out_ch == 3 || out_ch == 6), "hq step: 3-channel images, 3 or 6 model outputs");
   const int D = deg->img_dim;
   const long long img = 3LL * D * D, n = (long long)B * img;
+  HqRect r0{rects[0], rects[1], rects[2], rects[3], rects[4], rects[5]}, r1{rects[6], rects[7], rects[8], rects[9], rects[10], rects[11]};
+  for (const HqRect& r : {r0, r1})
+    if (r.h > 0) DDNM_CHECK(r.w > 0 && r.dy >= 0 && r.dx >= 0 && r.dy + r.h <= D && r.dx + r.w <= D && r.sy >= 0 && r.sx >= 0 &&
+                                r.sy + r.h <= canvas_h && r.sx + r.w <= canvas_w, "mask-shift rectangle out of range");
+  if (deg->image_mask) {
+    const HqMask q = hq_mask(deg);
+    const bool pool = q.S > 1 || q.gray;
+    const long long mo_stride = (long long)out_ch * D * D;
+    const unsigned grid = (unsigned)cdivll(n, 256);
+    if (pool) {
+      const long long ny = (long long)B * (q.gray ? 1 : 3) * (D / q.S) * (D / q.S);
+      hq_mask_A_kernel<true><<<(unsigned)cdivll(ny, 128), 128, 0, st>>>(x, model_out, mo_stride, *sc, q, scratch, B);
+    }
+    auto launch = [&](auto P, auto GEN) {
+      hq_mask_step_kernel<decltype(P)::value, decltype(GEN)::value><<<grid, 256, 0, st>>>(
+          x, model_out, mo_stride, q, scratch, apy, canvas, canvas_h, canvas_w, r0, r1, grad, noise.tape, *sc, x0_hat, x_next, n, noise);
+    };
+    if (pool) {
+      if (noise.tape) launch(std::true_type{}, std::false_type{});
+      else launch(std::true_type{}, std::true_type{});
+    } else {
+      if (noise.tape) launch(std::false_type{}, std::false_type{});
+      else launch(std::false_type{}, std::true_type{});
+    }
+    CUDA_CHECK(cudaGetLastError());
+    return;
+  }
   float* x0t = scratch;          // [n]
   float* apa = scratch + n;      // [n]
   float* yb = scratch + 2 * n;   // [<= n]
   hq_x0_kernel<<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, model_out, (long long)out_ch * D * D, sc->c_recip, sc->c_recipm1, sc->clip, x0t, img, n);
   simplified_A(deg, x0t, B, yb, st);
   simplified_Ap(deg, yb, B, apa, st);
-  HqRect r0{rects[0], rects[1], rects[2], rects[3], rects[4], rects[5]}, r1{rects[6], rects[7], rects[8], rects[9], rects[10], rects[11]};
-  for (const HqRect& r : {r0, r1})
-    if (r.h > 0) DDNM_CHECK(r.w > 0 && r.dy >= 0 && r.dx >= 0 && r.dy + r.h <= D && r.dx + r.w <= D && r.sy >= 0 && r.sx >= 0 &&
-                                r.sy + r.h <= canvas_h && r.sx + r.w <= canvas_w, "mask-shift rectangle out of range");
   if (noise.tape)
     hq_combine_kernel<false><<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, x0t, apa, apy, canvas, canvas_h, canvas_w, r0, r1, grad, noise.tape,
                                                                        *sc, x0_hat, x_next, 3, D, n, noise);
@@ -136,6 +262,24 @@ int ddnm_hq_canvas(const float* gt, int B, int H, int W, int scale, int use_gray
   DDNM_CHECK(gt && apy_canvas && B >= 1 && scale >= 1 && H % scale == 0 && W % scale == 0, "bad canvas geometry");
   const long long blocks = (long long)B * (H / scale) * (W / scale);
   hq_canvas_kernel<<<(unsigned)cdivll(blocks, 128), 128, 0, (cudaStream_t)stream>>>(gt, apy_canvas, B, H, W, scale, use_gray);
+  CUDA_CHECK(cudaGetLastError());
+  DDNM_API_END
+}
+
+int ddnm_hq_canvas_masked(const ddnm_simple_deg* deg, const float* gt, int B, float* apy, float* scratch, void* stream) {
+  DDNM_API_BEGIN
+  DDNM_CHECK(deg && deg->image_mask && gt && apy && scratch && B >= 1, "null argument");
+  const HqMask q = hq_mask(deg);
+  const bool pool = q.S > 1 || q.gray;
+  const cudaStream_t st = (cudaStream_t)stream;
+  const long long n = (long long)B * 3 * q.D * q.D;
+  if (pool) {
+    const long long ny = (long long)B * (q.gray ? 1 : 3) * (q.D / q.S) * (q.D / q.S);
+    hq_mask_A_kernel<false><<<(unsigned)cdivll(ny, 128), 128, 0, st>>>(gt, nullptr, 0, ddnm_hq_scalars{}, q, scratch, B);
+    hq_mask_canvas_kernel<true><<<(unsigned)cdivll(n, 256), 256, 0, st>>>(gt, q, scratch, apy, n);
+  } else {
+    hq_mask_canvas_kernel<false><<<(unsigned)cdivll(n, 256), 256, 0, st>>>(gt, q, nullptr, apy, n);
+  }
   CUDA_CHECK(cudaGetLastError());
   DDNM_API_END
 }

@@ -233,6 +233,7 @@ static SimpDeg make_deg(const ddnm_simple_deg* d) {
   DDNM_CHECK(d != nullptr, "null degradation");
   DDNM_CHECK(d->channels == 3 && d->img_dim > 0 && d->scale >= 1 && d->img_dim % d->scale == 0, "bad simplified degradation");
   DDNM_CHECK(!d->use_mask || d->mask != nullptr, "mask enabled but no mask given");
+  DDNM_CHECK(d->image_mask == nullptr, "per-image masks are read by the hq entry points only");
   SimpDeg g;
   g.use_mask = d->use_mask; g.use_gray = d->use_gray; g.scale = d->scale; g.D = d->img_dim; g.mask = d->mask;
   return g;

@@ -6,11 +6,19 @@ image — 256 x 256 windows every 128 pixels over an (H, W) canvas, each window 
     out = restore(model, y_img, classes, deg="sr_averagepooling", scale=4, sigma_y=0.0, resize_y=True,
                   timestep_respacing=100, schedule_jump_params=dict(t_T=100, n_sample=1, jump_length=10, jump_n_sample=3))
 
-``model`` is the class-conditional ``ddnm_b200.model.UNetModel`` (``create_model(class_cond=True, learn_sigma=True, ...)``, the
-imagenet 256x256 network of hq_demo/confs/inet256.yml); ``classes`` the ImageNet label(s) (main.py ``--class``); ``cond_fn`` the
-optional classifier gradient callable ``cond_fn(x, t, y)`` (main.py:65-76).  The loops are host code exactly as in the
-reference; every tensor operation of a step (x0_t, clipping, Eq. 17 / 19, the mask-shift overwrite, the posterior mean, the
-re-noising, the time-travel step) runs inside libddnm_b200.so, the denoiser as its CUDA graph.
+``model`` is a learn_sigma 256x256 ``ddnm_b200.model.UNetModel``: the class-conditional imagenet network of
+hq_demo/confs/inet256.yml (``classes``: the ImageNet label(s), main.py ``--class``) or the unconditional face network of
+hq_demo/confs/face256.yml (called without labels, main.py:98-100; ``classes`` may be None).  ``cond_fn`` is the optional
+classifier gradient callable ``cond_fn(x, t, y)`` (main.py:65-76).  ``conf_name`` selects the reference's ``conf.name`` gating:
+under ``"face256"`` the input must be 256 pixels high (:586-588) and the masked degradations ``inpainting`` / ``mask_color_sr``
+are available, with ``gt_keep_mask`` the (B,3,256,256) keep mask as the RePaint loader yields it (:601-621):
+
+    out = restore(model, gt, None, deg="inpainting", conf_name="face256", gt_keep_mask=mask, timestep_respacing=250,
+                  schedule_jump_params=dict(t_T=250, n_sample=1, jump_length=10, jump_n_sample=3))
+
+The loops are host code exactly as in the reference; every tensor operation of a step (x0_t, clipping, Eq. 17 / 19, the
+mask-shift overwrite, the posterior mean, the re-noising, the time-travel step) runs inside libddnm_b200.so, the denoiser as its
+CUDA graph.
 """
 import ctypes as C
 import math
@@ -19,7 +27,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .model import _EngineModel
+from .model import SuperResModel, UNetModel, _EngineModel
 from .noise import TAG_HQ, randn
 
 
@@ -138,27 +146,49 @@ def _shift_rects(sh, sw, sh_total, sw_total, H, W):
     return first, second
 
 
-def restore(model, gt, classes, deg="sr_averagepooling", scale=4, sigma_y=0.0, resize_y=False, timestep_respacing=100,
-            schedule_jump_params=None, diffusion_steps=1000, clip_denoised=True, cond_fn=None, noise=None, seed=None):
+def restore(model, gt, classes=None, deg="sr_averagepooling", scale=4, sigma_y=0.0, resize_y=False, timestep_respacing=100,
+            schedule_jump_params=None, diffusion_steps=1000, clip_denoised=True, cond_fn=None, noise=None, seed=None,
+            gt_keep_mask=None, conf_name="inet256"):
     """gt: the degraded input image(s) (B,3,h,w) in [-1,1] on the GPU (main.py:103-110); returns the restored canvas as a CPU
     tensor (B,3,H,W) — H, W = gt's size (x scale with ``resize_y``).  ``noise``: optional (n_draws,B,3,256,256) tape in the
     reference's draw order (initial x, then one per p_sample / undo call); by default the draws come from torch's generator in
     that order.  ``seed``: the library draws them instead (stream tag 3, draw index = position in that order, row = image), inside
     the step kernels; reproducible against itself, not against torch's generator.  The row is the image's index within this
     call (there is no row_offset), so with ``model.batch_invariant`` an image restores bit-identically in any call where it has
-    the same index, e.g. alone and as row 0 of a batch."""
+    the same index, e.g. alone and as row 0 of a batch.
+    ``conf_name``: "inet256" or "face256" (the reference's conf.name).  ``gt_keep_mask``: the keep mask of ``inpainting`` /
+    ``mask_color_sr`` (face256 only), fp32 in [0, 1] and broadcastable to (B,3,256,256); it multiplies, so fractional edge
+    values weigh the pixel.  The masked degradations restore one 256 x 256 window per image: ``resize_y`` with a scale above 1
+    would make gt larger than the mask, which the reference cannot multiply either.  hq_demo itself runs one image per call; with
+    B > 1 every degradation here works image by image (the reference's color2gray would fold the batch into channels)."""
     if seed is not None and noise is not None:
         raise ValueError("seed= and noise= are two sources for the same draws: give one")
+    if conf_name not in ("inet256", "face256"):
+        raise ValueError(f"conf_name must be 'inet256' or 'face256', not {conf_name!r}")
     if not isinstance(model, _EngineModel):
         model = getattr(model, "module", model)
-    if not isinstance(model, _EngineModel) or model.num_classes is None or model.out_ch != 6 or model.resolution != 256:
-        raise TypeError("hq.restore needs the class-conditional, learn_sigma 256x256 ddnm_b200 UNetModel")
+    if not isinstance(model, UNetModel) or isinstance(model, SuperResModel) or model.out_ch != 6 or model.resolution != 256:
+        raise TypeError("hq.restore needs a learn_sigma 256x256 ddnm_b200 UNetModel (class-conditional or unconditional)")
+    if model.num_classes is not None and classes is None:
+        raise ValueError("the class-conditional model needs classes")
     if 256 % scale != 0:
         raise ValueError("Please set a SR scale divisible by 256")
+    if conf_name == "face256" and gt.shape[2] != 256:             # :586-588, before resize_y
+        raise ValueError("Only support output size 256x256 for face images")
     table = {"sr_averagepooling": (0, scale), "colorization": (1, 1), "sr_color": (1, scale)}
+    if conf_name == "face256":                                  # :601-622
+        table.update(inpainting=(0, 1), mask_color_sr=(1, scale))
     if deg not in table:
         raise NotImplementedError("degradation type not supported")
     use_gray, sc = table[deg]
+    masked = deg in ("inpainting", "mask_color_sr")
+    if masked:
+        if gt_keep_mask is None:
+            raise ValueError(f"{deg} needs gt_keep_mask")
+        if resize_y and scale != 1:
+            raise ValueError(f"{deg} with resize_y: gt would be {256 * scale} pixels high, the keep mask is 256 x 256")
+        if gt.shape[3] != 256:
+            raise ValueError(f"{deg} needs a 256 x 256 gt (the keep mask's size)")
     L = _lib.lib()
     jump = schedule_jump_params or dict(t_T=int(timestep_respacing), n_sample=1, jump_length=10, jump_n_sample=3)
     K = SpacedTables(diffusion_steps, timestep_respacing)
@@ -173,13 +203,23 @@ def restore(model, gt, classes, deg="sr_averagepooling", scale=4, sigma_y=0.0, r
             raise ValueError("image size must be a multiple of the SR scale")
         if H < 256 or W < 256:
             raise ValueError("Please set a larger SR scale")
-        apy_canvas = torch.empty_like(gt)
-        _lib.check(L.ddnm_hq_canvas(_lib.ptr(gt), B, H, W, sc, use_gray, _lib.ptr(apy_canvas), _lib.cur_stream()))
-        final = torch.zeros_like(gt)
-        sh_total, sw_total = math.ceil(H / 128) - 1, math.ceil(W / 128) - 1
         d = _lib.SimpleDeg()
         d.use_mask, d.use_gray, d.scale, d.img_dim, d.channels, d.mask = 0, use_gray, sc, 256, 3, None
-        labels = torch.as_tensor(classes).to(dev).long().reshape(-1)
+        apy_canvas = torch.empty_like(gt)
+        scratch = torch.empty(3 * B * 3 * 256 * 256, device=dev)
+        if masked:
+            try:
+                mask = torch.broadcast_to(gt_keep_mask.to(dev).float(), (B, 3, 256, 256)).contiguous()
+            except RuntimeError as e:
+                raise ValueError(f"gt_keep_mask of shape {tuple(gt_keep_mask.shape)} does not broadcast to {(B, 3, 256, 256)}") from e
+            d.image_mask = mask.data_ptr()
+            _lib.check(L.ddnm_hq_canvas_masked(C.byref(d), _lib.ptr(gt), B, _lib.ptr(apy_canvas), _lib.ptr(scratch), _lib.cur_stream()))
+        else:
+            _lib.check(L.ddnm_hq_canvas(_lib.ptr(gt), B, H, W, sc, use_gray, _lib.ptr(apy_canvas), _lib.cur_stream()))
+        final = torch.zeros_like(gt)
+        sh_total, sw_total = math.ceil(H / 128) - 1, math.ceil(W / 128) - 1
+        labels = None if classes is None else torch.as_tensor(classes).to(dev).long().reshape(-1)
+        model_labels = labels if model.num_classes is not None else None     # face256: model(x, t, None) (main.py:98-100)
         tape = None if noise is None else noise.to(dev).float().contiguous()
         ns = None if seed is None else _lib.noise_seed(seed)
         draws = [0]
@@ -196,7 +236,6 @@ def restore(model, gt, classes, deg="sr_averagepooling", scale=4, sigma_y=0.0, r
         else:
             x = randn(seed, (B, 3, 256, 256), TAG_HQ, draw=draw(), device=dev)
         x_next, x0_hat = torch.empty_like(x), torch.empty_like(x)
-        scratch = torch.empty(3 * x.numel(), device=dev)
         times = get_schedule_jump(**jump)
         for sh in range(sh_total):
             for sw in range(sw_total):
@@ -209,7 +248,7 @@ def restore(model, gt, classes, deg="sr_averagepooling", scale=4, sigma_y=0.0, r
                     if t_cur < t_last:
                         t = t_last
                         t_model = torch.full((B,), float(K.timestep_map[t]), device=dev)
-                        mo = model(x, t_model, labels)
+                        mo = model(x, t_model, model_labels)
                         s = _lib.HqScalars()
                         f = np.float32
                         post_var = f(K.posterior_variance[t])

@@ -236,6 +236,10 @@ int ddnm_classifier_guidance_fn(void* user, int pair_index, int t, void* stream)
 typedef struct {
   int use_mask, use_gray, scale, img_dim, channels;
   const float* mask;          /* DEVICE [img_dim*img_dim] 0/1 (exp/inp_masks/mask.npy), NULL when use_mask == 0 */
+  /* appended: DEVICE [B,3,img_dim,img_dim] fp32 per-image, per-channel keep mask (hq_demo face256's gt_keep_mask, values in
+   * [0, 1]).  Only the hq entry points read it, with use_mask == 0: A(z) = pool(gray(z*image_mask)),
+   * Ap(v) = gray2color(upsample(v))*image_mask (pool / gray as scale / use_gray say).  NULL: no per-image mask. */
+  const float* image_mask;
 } ddnm_simple_deg;
 int ddnm_simplified_A(const ddnm_simple_deg* deg, const float* x, int B, float* y, void* stream);
 int ddnm_simplified_Ap(const ddnm_simple_deg* deg, const float* y, int B, float* x, void* stream);
@@ -261,6 +265,9 @@ int ddnm_sample_simplified_range_seeded(void* unet, const ddnm_simple_deg* deg, 
  *                   overwritten from the canvas (:344-384); mean = coef1*x0_hat + coef2*x (+ gamma_t*grad, :414-430);
  *                   x_next = mean + nonzero*sqrt(gamma_t)*noise.  scratch: 3*B*3*D*D floats.
  *   ddnm_hq_undo  : x = sqrt(1-beta)*x + sqrt(beta)*noise (time-travel back step)
+ * With deg->image_mask set (face256's inpainting: scale 1, no gray; mask_color_sr: gray, scale s) the step reads the mask of each
+ * row and computes x0_t, Ap(A(x0_t)) and the rest in one fused pass (plus one pooling pass when scale > 1 or gray), with
+ * scratch >= B*3*D*D/scale^2 floats; ddnm_hq_canvas_masked gives that degradation's Apy = Ap(A(gt)) for gt (B,3,D,D).
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
   float c_recip, c_recipm1;   /* sqrt_recip_alphas_cumprod[t], sqrt_recipm1_alphas_cumprod[t] */
@@ -281,6 +288,9 @@ int ddnm_hq_step_seeded(const ddnm_simple_deg* deg, const float* x, const float*
                         float* scratch, void* stream);
 int ddnm_hq_undo_seeded(float* x, const ddnm_noise_seed* seed, unsigned draw, float sqrt_one_minus_beta, float sqrt_beta, int B,
                         long long per_image, void* stream);
+/* Apy = Ap(A(gt)) of a degradation with deg->image_mask (A_temp = A, :601-622, :645-646); gt, apy [B,3,img_dim,img_dim];
+ * scratch >= B*3*D*D/scale^2 floats */
+int ddnm_hq_canvas_masked(const ddnm_simple_deg* deg, const float* gt, int B, float* apy, float* scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * The runner's I/O step either side of the loop (guided_diffusion/diffusion.py:533-603), device pointers throughout.
