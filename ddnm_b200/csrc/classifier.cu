@@ -419,11 +419,6 @@ __global__ void __launch_bounds__(128) stem_bwd_kernel(const float* __restrict__
   for (int ci = 0; ci < CIN; ++ci) dx[(((size_t)n * CIN + ci) * H + y) * W + x] = acc[ci] * sc;
 }
 
-__global__ void fill_f32_kernel(float* p, int n, float v) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = v;
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // program
 // ---------------------------------------------------------------------------------------------------------------
@@ -674,8 +669,7 @@ void UNetEncoder::build_program() {
   alloc_common(act_max, 0);
   alloc_attention(att_qkv, att_S, att_O);
   scale_in_ = (float*)arena_.alloc(4);
-  fill_f32_kernel<<<1, 32>>>(scale_in_, 1, 1.0f);   // the scale of an eager profile run before any grad() call
-  CUDA_CHECK(cudaGetLastError());
+  fill(scale_in_, 1, 1.0f, 0);   // the scale of an eager profile run before any grad() call
   grad_ = (float*)arena_.alloc((size_t)B_ * in_ch_ * R * R * 4);
   for (float*& g : gx_) g = (float*)arena_.alloc(act_max * 4);
   g1_ = (float*)arena_.alloc(act_max * 4);
@@ -742,11 +736,6 @@ void UNetEncoder::check_labels(const int* labels, cudaStream_t stream) const {
                "label " + std::to_string(hl[i]) + " outside [0, " + std::to_string(cfg_.out_channels) + ")");
 }
 
-void UNetEncoder::fill_t(float t, cudaStream_t stream) {
-  fill_f32_kernel<<<cdiv(B_, 128), 128, 0, stream>>>(t_in_, B_, t);
-  CUDA_CHECK(cudaGetLastError());
-}
-
 void UNetEncoder::grad(const float* x, const float* t, const int* labels, float scale, float* grad_out, float* logits, cudaStream_t stream,
                        bool labels_checked) {
   DDNM_CHECK(finalized_, "classifier gradient before finalize");
@@ -756,8 +745,7 @@ void UNetEncoder::grad(const float* x, const float* t, const int* labels, float 
   if (x != x_in_) CUDA_CHECK(cudaMemcpyAsync(x_in_, x, xin, cudaMemcpyDeviceToDevice, stream));
   if (t != t_in_) CUDA_CHECK(cudaMemcpyAsync(t_in_, t, (size_t)B_ * 4, cudaMemcpyDeviceToDevice, stream));
   if (labels != labels_in_) CUDA_CHECK(cudaMemcpyAsync(labels_in_, labels, (size_t)B_ * sizeof(int), cudaMemcpyDeviceToDevice, stream));
-  fill_f32_kernel<<<1, 32, 0, stream>>>(scale_in_, 1, scale);
-  CUDA_CHECK(cudaGetLastError());
+  fill(scale_in_, 1, scale, stream);
   replay(stream, ops_.size(), ggraph_, ggraph_exec_);
   CUDA_CHECK(cudaMemcpyAsync(grad_out, grad_, xin, cudaMemcpyDeviceToDevice, stream));
   if (logits) CUDA_CHECK(cudaMemcpyAsync(logits, out_, out_elems() * 4, cudaMemcpyDeviceToDevice, stream));

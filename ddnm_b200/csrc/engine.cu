@@ -482,6 +482,8 @@ void UNetEngine::run_ops(cudaStream_t s, size_t n) {
   for (size_t i = 0; i < n && i < ops_.size(); ++i) ops_[i].run(s);
 }
 
+void UNetEngine::fill_t(float t, cudaStream_t stream) { fill(t_in_, B_, t, stream); }
+
 void UNetEngine::set_labels(const int* labels_dev, cudaStream_t stream) {
   DDNM_CHECK(class_cond_, "set_labels on a network without a label embedding");
   DDNM_CHECK(labels_dev != nullptr, "null labels");

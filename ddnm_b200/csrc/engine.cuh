@@ -82,6 +82,8 @@ class UNetEngine {
   int resolution() const { return R_; }
   float* x_in() const { return x_in_; }
   float* t_in() const { return t_in_; }
+  // t_in() = t for every image, on the device
+  void fill_t(float t, cudaStream_t stream);
   // class labels of the next forward (device int32 [B]); only meaningful for class-conditional networks
   int* labels_in() const { return labels_in_; }
   bool class_conditional() const { return class_cond_; }
@@ -254,8 +256,6 @@ class UNetEncoder : public UNetEngine {
             bool labels_checked = false);
   // throws unless every label is in [0, out_channels); reads them to the host (synchronises `stream`)
   void check_labels(const int* labels, cudaStream_t stream) const;
-  // t_in() = t for every image, on the device
-  void fill_t(float t, cudaStream_t stream);
   int num_classes() const { return cfg_.out_channels; }
 
  private:

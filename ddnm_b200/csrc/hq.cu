@@ -9,13 +9,9 @@
 
 #include "../../include/ddnm_b200.h"
 #include "api_util.cuh"
-#include "common.cuh"
-#include "noise.cuh"
+#include "operators.cuh"
 
 namespace ddnm {
-// simplified.cu: A / Ap of the image-space operators on (B, 3, D, D) images
-void simplified_A(const ddnm_simple_deg* d, const float* x, int B, float* y, cudaStream_t st);
-void simplified_Ap(const ddnm_simple_deg* d, const float* y, int B, float* x, cudaStream_t st);
 
 // x0_t = clamp(sqrt_recip_alphas_cumprod*x - sqrt_recipm1_alphas_cumprod*eps, -1, 1)       (:404-411, :296-300)
 __global__ void hq_x0_kernel(const float* __restrict__ x, const float* __restrict__ mo, long long mo_stride, float c_recip, float c_recipm1,
@@ -157,22 +153,6 @@ __global__ void hq_mask_canvas_kernel(const float* __restrict__ gt, HqMask q, co
   apy[i] = hq_mask_ApA<POOL>(q, y, gt[i], i, b, (int)(r / HW), (int)((r / D) % D), (int)(r % D));
 }
 
-// x = sqrt(1 - beta)*x + sqrt(beta)*noise            (:211-217)
-template <bool GEN>   // GEN: the draw is generated in registers from gen (img = elements per image), z unused
-__global__ void hq_undo_kernel(float* __restrict__ x, const float* __restrict__ z, float a, float b, long long n, long long img,
-                               NoiseSrc gen) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float zi;
-  if (GEN) {
-    const long long r = i / img;
-    zi = noise_at(gen, (int)r, i - r * img);
-  } else {
-    zi = z[i];
-  }
-  x[i] = __fadd_rn(__fmul_rn(a, x[i]), __fmul_rn(b, zi));
-}
-
 // canvas preparation: Apy_temp = Ap(A_temp(gt)) for gt (B, 3, H, W): block means (optionally of the gray image) broadcast back
 __global__ void hq_canvas_kernel(const float* __restrict__ gt, float* __restrict__ out, int B, int H, int W, int scale, int use_gray) {
   const int yd = H / scale, xd = W / scale;
@@ -227,17 +207,14 @@ static void hq_step(const ddnm_simple_deg* deg, const float* x, const float* mod
       const long long ny = (long long)B * (q.gray ? 1 : 3) * (D / q.S) * (D / q.S);
       hq_mask_A_kernel<true><<<(unsigned)cdivll(ny, 128), 128, 0, st>>>(x, model_out, mo_stride, *sc, q, scratch, B);
     }
-    auto launch = [&](auto P, auto GEN) {
-      hq_mask_step_kernel<decltype(P)::value, decltype(GEN)::value><<<grid, 256, 0, st>>>(
-          x, model_out, mo_stride, q, scratch, apy, canvas, canvas_h, canvas_w, r0, r1, grad, noise.tape, *sc, x0_hat, x_next, n, noise);
+    auto launch = [&](auto P) {
+      noise_dispatch(noise, [&](auto gen) {
+        hq_mask_step_kernel<decltype(P)::value, decltype(gen)::value><<<grid, 256, 0, st>>>(
+            x, model_out, mo_stride, q, scratch, apy, canvas, canvas_h, canvas_w, r0, r1, grad, noise.tape, *sc, x0_hat, x_next, n, noise);
+      });
     };
-    if (pool) {
-      if (noise.tape) launch(std::true_type{}, std::false_type{});
-      else launch(std::true_type{}, std::true_type{});
-    } else {
-      if (noise.tape) launch(std::false_type{}, std::false_type{});
-      else launch(std::false_type{}, std::true_type{});
-    }
+    if (pool) launch(std::true_type{});
+    else launch(std::false_type{});
     CUDA_CHECK(cudaGetLastError());
     return;
   }
@@ -247,12 +224,10 @@ static void hq_step(const ddnm_simple_deg* deg, const float* x, const float* mod
   hq_x0_kernel<<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, model_out, (long long)out_ch * D * D, sc->c_recip, sc->c_recipm1, sc->clip, x0t, img, n);
   simplified_A(deg, x0t, B, yb, st);
   simplified_Ap(deg, yb, B, apa, st);
-  if (noise.tape)
-    hq_combine_kernel<false><<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, x0t, apa, apy, canvas, canvas_h, canvas_w, r0, r1, grad, noise.tape,
-                                                                       *sc, x0_hat, x_next, 3, D, n, noise);
-  else
-    hq_combine_kernel<true><<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, x0t, apa, apy, canvas, canvas_h, canvas_w, r0, r1, grad, nullptr,
-                                                                      *sc, x0_hat, x_next, 3, D, n, noise);
+  noise_dispatch(noise, [&](auto gen) {
+    hq_combine_kernel<decltype(gen)::value><<<(unsigned)cdivll(n, 256), 256, 0, st>>>(
+        x, x0t, apa, apy, canvas, canvas_h, canvas_w, r0, r1, grad, noise.tape, *sc, x0_hat, x_next, 3, D, n, noise);
+  });
   CUDA_CHECK(cudaGetLastError());
 }
 
@@ -306,20 +281,16 @@ int ddnm_hq_step_seeded(const ddnm_simple_deg* deg, const float* x, const float*
 int ddnm_hq_undo(float* x, const float* noise, float sqrt_one_minus_beta, float sqrt_beta, long long n, void* stream) {
   DDNM_API_BEGIN
   DDNM_CHECK(x && noise && n > 0, "null argument");
-  hq_undo_kernel<false><<<(unsigned)cdivll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, noise, sqrt_one_minus_beta, sqrt_beta, n, n,
-                                                                                     NoiseSrc{});
-  CUDA_CHECK(cudaGetLastError());
+  // x = sqrt(1 - beta)*x + sqrt(beta)*noise            (:211-217)
+  renoise(x, sqrt_one_minus_beta, sqrt_beta, noise_tape(noise), x, n, n, (cudaStream_t)stream);
   DDNM_API_END
 }
 int ddnm_hq_undo_seeded(float* x, const ddnm_noise_seed* seed, unsigned draw, float sqrt_one_minus_beta, float sqrt_beta, int B,
                         long long per_image, void* stream) {
   DDNM_API_BEGIN
   DDNM_CHECK(x && B >= 1 && per_image > 0, "null argument");
-  const NoiseSrc gen = noise_seeded(seed, NZ_HQ, draw, B);
-  const long long n = (long long)B * per_image;
-  hq_undo_kernel<true><<<(unsigned)cdivll(n, 256), 256, 0, (cudaStream_t)stream>>>(x, nullptr, sqrt_one_minus_beta, sqrt_beta, n,
-                                                                                    per_image, gen);
-  CUDA_CHECK(cudaGetLastError());
+  renoise(x, sqrt_one_minus_beta, sqrt_beta, noise_seeded(seed, NZ_HQ, draw, B), x, (long long)B * per_image, per_image,
+          (cudaStream_t)stream);
   DDNM_API_END
 }
 }

@@ -889,6 +889,15 @@ void sinusoid(const float* t, int N, const float* freq, int dim, bool sin_first,
   CUDA_CHECK(cudaGetLastError());
 }
 
+__global__ void fill_kernel(float* p, int n, float v) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) p[i] = v;
+}
+void fill(float* p, int n, float v, cudaStream_t st) {
+  fill_kernel<<<cdiv(n, 128), 128, 0, st>>>(p, n, v);
+  CUDA_CHECK(cudaGetLastError());
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Batched fp32 GEMM, 64x64x16 tiles, 4x4 per thread (torch.bmm in AttnBlock, models.py:177,185).
 // ---------------------------------------------------------------------------------------------------------------

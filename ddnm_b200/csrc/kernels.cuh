@@ -45,6 +45,8 @@ void linear(const float* in, int N, int K, const float* W, const float* bias, in
 void add_label_swish(float* v, const float* table, const int* labels, int N, int D, int num_classes, cudaStream_t s);
 // emb[n][:] = [sin(t*f) | cos(t*f)] (sin_first) or [cos | sin]; f has dim/2 entries
 void sinusoid(const float* t, int N, const float* freq, int dim, bool sin_first, float* emb, cudaStream_t s);
+// p[0..n) = v
+void fill(float* p, int n, float v, cudaStream_t s);
 
 // batched fp32 GEMM on CUDA cores (attention at small token counts).
 //   NT: C[b][m][n] = alpha * sum_k A[b][m][k] * B[b][n][k];   NN: ... * B[b][k][n]

@@ -1,6 +1,6 @@
 // Materialised form of the generator of noise.cuh: what a caller uses for x_T and the measurement noise, what the operators
 // whose Lambda_noise is a transform (not a map) fill their one-pair scratch with, and what the tests compare the in-register
-// consumers against.
+// consumers against.  Also the one elementwise consumer shared by the loops: the re-noise a*x + b*z.
 #include "noise.cuh"
 
 #include "../../include/ddnm_b200.h"
@@ -27,6 +27,28 @@ __global__ void noise_fill_kernel(NoiseSrc z, float* __restrict__ out, long long
 void noise_fill(const NoiseSrc& z, float* out, int B, long long per_image, cudaStream_t st) {
   const long long quads = (per_image + 3) / 4, total = quads * B;
   noise_fill_kernel<<<(unsigned)cdivll(total, 256), 256, 0, st>>>(z, out, per_image, quads, total);
+  CUDA_CHECK(cudaGetLastError());
+}
+
+// x and out may alias (the in-place undo), so neither is __restrict__
+template <bool GEN>
+__global__ void renoise_kernel(const float* x, float a, float b, NoiseSrc z, float* out, long long n, long long img) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float zi;
+  if (GEN) {
+    const long long r = i / img;
+    zi = noise_at(z, (int)r, i - r * img);
+  } else {
+    zi = z.tape[i];
+  }
+  out[i] = __fadd_rn(__fmul_rn(a, x[i]), __fmul_rn(b, zi));
+}
+
+void renoise(const float* x, float a, float b, const NoiseSrc& z, float* out, long long n, long long img, cudaStream_t st) {
+  noise_dispatch(z, [&](auto gen) {
+    renoise_kernel<decltype(gen)::value><<<(unsigned)cdivll(n, 256), 256, 0, st>>>(x, a, b, z, out, n, img);
+  });
   CUDA_CHECK(cudaGetLastError());
 }
 

@@ -9,6 +9,7 @@
 // oracle/noise.py states the same in numpy.
 #pragma once
 #include <cstdint>
+#include <type_traits>
 
 #include <cuda_runtime.h>
 
@@ -70,14 +71,18 @@ __device__ __forceinline__ float noise_at(const NoiseSrc& z, int row, long long 
   const float2 v = noise_pair(z, row, elem >> 1);
   return (elem & 1) ? v.y : v.x;
 }
-// GEN is a template parameter of every consumer, so the tape form of a kernel is the plain load it always was
-template <bool GEN>
-__device__ __forceinline__ float noise_get(const NoiseSrc& z, int row, long long elem, long long img) {
-  if (GEN) return noise_at(z, row, elem);
-  return z.tape[(long long)row * img + elem];
+// Every consumer kernel takes GEN as a template parameter, so its tape form is the plain load it always was.  A launch site picks
+// the instantiation here: f(std::bool_constant<GEN>{}) with GEN = the draws are generated (no tape).
+template <class F>
+inline void noise_dispatch(const NoiseSrc& z, F&& f) {
+  if (z.tape) f(std::false_type{});
+  else f(std::true_type{});
 }
 
 // out[b][e] = the generated value of element e of image row0 + b  (ddnm_noise_fill; also fills an operator's one-pair scratch)
 void noise_fill(const NoiseSrc& z, float* out, int B, long long per_image, cudaStream_t st);
+// out[i] = a*x[i] + b*z[i] over n elements, img per image row: the samplers' time-travel re-noise and hq_demo's _undo.
+// out == x is allowed.
+void renoise(const float* x, float a, float b, const NoiseSrc& z, float* out, long long n, long long img, cudaStream_t st);
 
 }  // namespace ddnm

@@ -272,21 +272,17 @@ __global__ void __launch_bounds__(128) local_kernel(const float* __restrict__ in
 template <int K, int MODE>
 static void local_launch(int fn, const float* in0, const float* in1, long long in1_stride, const float* in2, const float* y,
                          const float* V, float u00, float s0, const StepScalars& sc, float* out0, float* out1, long long groups,
-                         int C, int D, cudaStream_t st, const NoiseSrc* gen = nullptr) {
+                         int C, int D, cudaStream_t st, const NoiseSrc& noise) {
   const int grid = (int)cdivll(groups, 128);
-  const NoiseSrc g = gen ? *gen : NoiseSrc{};
 #define LL(F, GEN) \
-  local_kernel<K, MODE, F, GEN><<<grid, 128, 0, st>>>(in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, g)
+  local_kernel<K, MODE, F, GEN><<<grid, 128, 0, st>>>(in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, noise)
   switch (fn) {
     case LF_A: LL(LF_A, false); break;
     case LF_PINV: LL(LF_PINV, false); break;
     case LF_PROJECT: LL(LF_PROJECT, false); break;
     case LF_LAMBDA: LL(LF_LAMBDA, false); break;
     case LF_NOISE: LL(LF_NOISE, false); break;
-    default:
-      if (gen) LL(LF_STEP, true);
-      else LL(LF_STEP, false);
-      break;
+    default: noise_dispatch(noise, [&](auto gen) { LL(LF_STEP, decltype(gen)::value); }); break;
   }
 #undef LL
   CUDA_CHECK(cudaGetLastError());
@@ -736,14 +732,14 @@ static inline int blocks(long long n, int t = 256) { return (int)cdivll(n, t); }
 template <int FN>
 static void local_dispatch(int kind, int ratio, const float* in0, const float* in1, long long in1_stride, const float* in2,
                            const float* y, const float* V, float u00, float s0, const StepScalars& sc, float* out0, float* out1,
-                           int B, int C, int D, cudaStream_t st, const NoiseSrc* gen = nullptr) {
+                           int B, int C, int D, cudaStream_t st, const NoiseSrc& noise = NoiseSrc{}) {   // noise: LF_STEP's draws
   if (kind == OP_COLOR) {
-    local_launch<3, 1>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, (long long)B * D * D, C, D, st, gen);
+    local_launch<3, 1>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, (long long)B * D * D, C, D, st, noise);
   } else {
     const long long groups = (long long)B * C * (D / ratio) * (D / ratio);
-    if (ratio == 2) local_launch<4, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, gen);
-    else if (ratio == 4) local_launch<16, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, gen);
-    else local_launch<64, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, gen);
+    if (ratio == 2) local_launch<4, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, noise);
+    else if (ratio == 4) local_launch<16, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, noise);
+    else local_launch<64, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, noise);
   }
 }
 
@@ -1185,16 +1181,17 @@ void Operator::step(const float* xt, const float* et, long long et_stride, const
   const long long img = N_;
   const long long n = (long long)B * img;
   const float* noise = nz.tape;
-  const bool gen = noise == nullptr;
   if ((kind_ == OP_SR && !sr_generic_) || kind_ == OP_COLOR) {
-    local_dispatch<LF_STEP>(kind_, ratio_, xt, et, et_stride, noise, y, V_, u00_, s0_, sc, x0_t, xt_next, B, C_, D_, s,
-                            gen ? &nz : nullptr);
+    local_dispatch<LF_STEP>(kind_, ratio_, xt, et, et_stride, noise, y, V_, u00_, s0_, sc, x0_t, xt_next, B, C_, D_, s, nz);
   } else if (kind_ == OP_INPAINT) {
-    if (gen) inpaint_kernel<LF_STEP, true><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, nullptr, y, rank_, sc, x0_t, xt_next, B, C_, n2, M_, nz);
-    else inpaint_kernel<LF_STEP><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, rank_, sc, x0_t, xt_next, B, C_, n2, M_, nz);
+    noise_dispatch(nz, [&](auto gen) {
+      inpaint_kernel<LF_STEP, decltype(gen)::value><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, rank_, sc, x0_t, xt_next, B,
+                                                                              C_, n2, M_, nz);
+    });
   } else if (kind_ == OP_DENOISE) {
-    if (gen) denoise_kernel<LF_STEP, true><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, nullptr, y, sc, x0_t, xt_next, B, img, nz);
-    else denoise_kernel<LF_STEP><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, sc, x0_t, xt_next, B, img, nz);
+    noise_dispatch(nz, [&](auto gen) {
+      denoise_kernel<LF_STEP, decltype(gen)::value><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, sc, x0_t, xt_next, B, img, nz);
+    });
   } else {
     // generic path: x0_t, residual r = A^+(A x0_t - y), then the DDNM / DDNM+ update
     float* et3 = scratch(5, n);
@@ -1219,10 +1216,11 @@ void Operator::step(const float* xt, const float* et, long long et_stride, const
       }
     }
     if (!sc.use_plus) {
-      if (gen) final_ddnm_kernel<true><<<blocks(n), 256, 0, s>>>(x0_t, R, nullptr, et3, sc, xt_next, n, img, nz);
-      else final_ddnm_kernel<false><<<blocks(n), 256, 0, s>>>(x0_t, R, noise, et3, sc, xt_next, n, img, nz);
+      noise_dispatch(nz, [&](auto gen) {
+        final_ddnm_kernel<decltype(gen)::value><<<blocks(n), 256, 0, s>>>(x0_t, R, noise, et3, sc, xt_next, n, img, nz);
+      });
     } else {
-      if (gen) {
+      if (!noise) {
         // Lambda_noise of these operators is a transform of the whole draw (a GEMM or a Walsh-Hadamard transform of the raw
         // pixels), not a map: materialise this ONE pair's draws, the same values the fused kernels make in registers
         float* Z = scratch(10, (size_t)n);

@@ -83,4 +83,18 @@ class Operator {
   size_t scr_elems_[11] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // [10]: one pair of generated draws (step, seeded DDNM+)
 };
 
+// simplified.cu: the runner's image-space degradations (mask / colour-to-gray / average-pool, diffusion.py:244-290) on
+// (B, 3, D, D) images
+struct SimpDeg {
+  int use_mask, use_gray, scale, D;
+  const float* mask;
+};
+SimpDeg make_deg(const ddnm_simple_deg* d);   // throws on a malformed degradation
+void simplified_A(const ddnm_simple_deg* d, const float* x, int B, float* y, cudaStream_t st);
+void simplified_Ap(const ddnm_simple_deg* d, const float* y, int B, float* x, cudaStream_t st);
+// One pair of the simplified DDNM+ loop: x0_t -> x0t, the Eq. 17 / 19 update -> xt_next, with sc's DDIM terms and lambda_t, gamma_t
+// derived from at_next and sigma_y (diffusion.py:355-381).  noise: a tape of this pair's draws or a generated source.
+void simplified_step(const SimpDeg& dg, const float* xt, const float* et, long long et_stride, const NoiseSrc& noise, const float* y,
+                     int B, const StepScalars& sc, float at_next, float sigma_y, float* x0t, float* xt_next, cudaStream_t st);
+
 }  // namespace ddnm

@@ -1,22 +1,17 @@
 // The "simplified" DDNM+ loop of the reference runner (guided_diffusion/diffusion.py:211-415, README quick start):
 // image-space operators built from mask / colour-to-gray / average-pool (diffusion.py:244-290, helpers :27-42) and a scalar
 // lambda_t / gamma_t update (:355-376).  One fused kernel per step; thread = one scale x scale patch across the 3 channels.
+// The loop around the step is the SVD samplers' sample_range (sampler.cu).
 #include <cmath>
-#include <memory>
 
 #include "../../include/ddnm_b200.h"
 #include "api_util.cuh"
-#include "engine.cuh"
-#include "noise.cuh"
+#include "operators.cuh"
 
 namespace ddnm {
 
 struct SimpScalars {
   float sqrt_at, sqrt_1m_at, sqrt_atn, c1, c2, lambda_t, gamma_t;
-};
-struct SimpDeg {
-  int use_mask, use_gray, scale, D;
-  const float* mask;
 };
 
 enum { SF_A = 0, SF_AP = 1, SF_STEP = 2 };
@@ -229,7 +224,7 @@ static void simp_launch(const SimpDeg& dg, const float* in0, const float* et, lo
   CUDA_CHECK(cudaGetLastError());
 }
 
-static SimpDeg make_deg(const ddnm_simple_deg* d) {
+SimpDeg make_deg(const ddnm_simple_deg* d) {
   DDNM_CHECK(d != nullptr, "null degradation");
   DDNM_CHECK(d->channels == 3 && d->img_dim > 0 && d->scale >= 1 && d->img_dim % d->scale == 0, "bad simplified degradation");
   DDNM_CHECK(!d->use_mask || d->mask != nullptr, "mask enabled but no mask given");
@@ -239,103 +234,24 @@ static SimpDeg make_deg(const ddnm_simple_deg* d) {
   return g;
 }
 
-__global__ void simp_fill_kernel(float* p, int n, float v) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = v;
-}
-template <bool GEN>   // GEN: the draw is generated in registers from gen (img = elements per image), z unused
-__global__ void simp_travel_kernel(const float* __restrict__ x0, const float* __restrict__ z, float sa, float s1, float* __restrict__ xn,
-                                   long long n, long long img, NoiseSrc gen) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float zi;
-  if (GEN) {
-    const long long b = i / img;
-    zi = noise_at(gen, (int)b, i - b * img);
+void simplified_step(const SimpDeg& dg, const float* xt, const float* et, long long et_stride, const NoiseSrc& noise, const float* y,
+                     int B, const StepScalars& sc, float at_next, float sigma_y, float* x0t, float* xt_next, cudaStream_t st) {
+  SimpScalars s{sc.sqrt_at, sc.sqrt_1m_at, sc.sqrt_atn, sc.c1, sc.c2, 0.0f, 0.0f};
+  // Eq. 19 with the runner's sigma_t = sqrt(1 - at_next**2)  (diffusion.py:356, :366-371)
+  const float sigma_t = std::sqrt(1.0f - at_next * at_next);
+  const float asy = at_next * sigma_y;
+  if (sigma_t >= asy) {
+    s.lambda_t = 1.0f;
+    s.gamma_t = std::sqrt(sigma_t * sigma_t - asy * asy);
   } else {
-    zi = z[i];
+    s.lambda_t = sigma_t / asy;
+    s.gamma_t = 0.0f;
   }
-  xn[i] = __fadd_rn(__fmul_rn(sa, x0[i]), __fmul_rn(zi, s1));
+  noise_dispatch(noise, [&](auto gen) {
+    simp_launch<SF_STEP, decltype(gen)::value>(dg, xt, et, et_stride, noise.tape, y, s, x0t, xt_next, B, st, noise);
+  });
 }
 
-// pairs [k0, k1) with the state in the caller's buffers (same contract as sample_range in sampler.cu)
-static void sample_simplified_range(UNetEngine* unet, const ddnm_simple_deg* d, const ddnm_schedule* sc, int k0, int k1, float* xt_state,
-                                    float* x0t, int* have_x0, const float* y, const NoiseSrc& noise, int B, cudaStream_t st) {
-  DDNM_CHECK(unet && sc && xt_state && x0t && have_x0 && y, "null argument");
-  DDNM_CHECK(unet->batch() == B, "engine was built for a different batch size");
-  DDNM_CHECK(0 <= k0 && k0 <= k1 && k1 <= sc->n_pairs, "pair range outside the schedule");
-  SimpDeg dg = make_deg(d);
-  const int R = unet->resolution();
-  DDNM_CHECK(dg.D == R && unet->in_channels() == 3, "degradation / denoiser image size mismatch");
-  const long long n = (long long)B * 3 * R * R;
-  const long long et_stride = (long long)unet->out_ch() * R * R;
-  float* xt = unet->x_in();
-  float* et = unet->out_buf();
-  StreamBuf xnb((size_t)n, st);
-  float* xn = xnb.p;
-  CUDA_CHECK(cudaMemcpyAsync(xt, xt_state, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  const float eta = sc->eta, sigma_y = sc->sigma_y;
-  const float c_eta = (float)std::sqrt(1.0 - (double)eta * (double)eta);
-  for (int k = k0; k < k1; ++k) {
-    const int i = sc->t_i[k], j = sc->t_j[k];
-    DDNM_CHECK(i >= 0 && i < sc->num_timesteps && j >= -1 && j < sc->num_timesteps, "time index out of range");
-    const float at_next = sc->abar[j + 1];
-    NoiseSrc z = noise;   // a tape holds the draws of exactly these pairs; a generated source is indexed by the pair
-    if (z.tape) z.tape += (long long)(k - k0) * n;
-    else z.draw = (unsigned)k;
-    if (j < i) {
-      const float at = sc->abar[i + 1];
-      simp_fill_kernel<<<cdiv(B, 128), 128, 0, st>>>(unet->t_in(), B, (float)i);
-      unet->forward(xt, unet->t_in(), et, st);
-      SimpScalars s{};
-      s.sqrt_at = std::sqrt(at);
-      s.sqrt_1m_at = std::sqrt(1.0f - at);
-      s.sqrt_atn = std::sqrt(at_next);
-      const float s1n = std::sqrt(1.0f - at_next);
-      s.c1 = s1n * eta;
-      s.c2 = s1n * c_eta;
-      // Eq. 19 with the runner's sigma_t = sqrt(1 - at_next**2)  (diffusion.py:356, :366-371)
-      const float sigma_t = std::sqrt(1.0f - at_next * at_next);
-      const float asy = at_next * sigma_y;
-      if (sigma_t >= asy) {
-        s.lambda_t = 1.0f;
-        s.gamma_t = std::sqrt(sigma_t * sigma_t - asy * asy);
-      } else {
-        s.lambda_t = sigma_t / asy;
-        s.gamma_t = 0.0f;
-      }
-      if (z.tape) simp_launch<SF_STEP>(dg, xt, et, et_stride, z.tape, y, s, x0t, xn, B, st);
-      else simp_launch<SF_STEP, true>(dg, xt, et, et_stride, nullptr, y, s, x0t, xn, B, st, z);
-      *have_x0 = 1;
-    } else {
-      DDNM_CHECK(*have_x0, "schedule starts with a travel-back step");
-      const float sa = std::sqrt(at_next), s1 = std::sqrt(1.0f - at_next);
-      if (z.tape) simp_travel_kernel<false><<<(int)cdivll(n, 256), 256, 0, st>>>(x0t, z.tape, sa, s1, xn, n, 3LL * R * R, z);
-      else simp_travel_kernel<true><<<(int)cdivll(n, 256), 256, 0, st>>>(x0t, nullptr, sa, s1, xn, n, 3LL * R * R, z);
-      CUDA_CHECK(cudaGetLastError());
-    }
-    CUDA_CHECK(cudaMemcpyAsync(xt, xn, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  }
-  CUDA_CHECK(cudaMemcpyAsync(xt_state, xt, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
-}
-
-static void sample_simplified(UNetEngine* unet, const ddnm_simple_deg* d, const ddnm_schedule* sc, const float* x_T, const float* y,
-                              const float* noise, int B, float* out_x0, float* out_x0_pred, cudaStream_t st) {
-  DDNM_CHECK(unet && sc && x_T && y && noise && out_x0, "null argument");
-  DDNM_CHECK(unet->batch() == B, "engine was built for a different batch size");
-  const long long n = (long long)B * 3 * unet->resolution() * unet->resolution();
-  std::unique_ptr<StreamBuf> own;
-  float* x0t = out_x0_pred;
-  if (!x0t) {
-    own.reset(new StreamBuf((size_t)n, st));
-    x0t = own->p;
-  }
-  if (out_x0 != x_T) CUDA_CHECK(cudaMemcpyAsync(out_x0, x_T, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  int have_x0 = 0;
-  sample_simplified_range(unet, d, sc, 0, sc->n_pairs, out_x0, x0t, &have_x0, y, noise_tape(noise), B, st);
-}
-
-// used by the hq_demo mask-shift step (hq.cu)
 void simplified_A(const ddnm_simple_deg* d, const float* x, int B, float* y, cudaStream_t st) {
   SimpScalars s{};
   simp_launch<SF_A>(make_deg(d), x, nullptr, 0, nullptr, nullptr, s, y, nullptr, B, st);
@@ -351,36 +267,12 @@ using namespace ddnm;
 extern "C" {
 int ddnm_simplified_A(const ddnm_simple_deg* d, const float* x, int B, float* y, void* stream) {
   DDNM_API_BEGIN
-  SimpScalars s{};
-  simp_launch<SF_A>(make_deg(d), x, nullptr, 0, nullptr, nullptr, s, y, nullptr, B, (cudaStream_t)stream);
+  simplified_A(d, x, B, y, (cudaStream_t)stream);
   DDNM_API_END
 }
 int ddnm_simplified_Ap(const ddnm_simple_deg* d, const float* y, int B, float* x, void* stream) {
   DDNM_API_BEGIN
-  SimpScalars s{};
-  simp_launch<SF_AP>(make_deg(d), nullptr, nullptr, 0, nullptr, y, s, x, nullptr, B, (cudaStream_t)stream);
-  DDNM_API_END
-}
-int ddnm_sample_simplified_range(void* unet, const ddnm_simple_deg* d, const ddnm_schedule* sched, int k_begin, int k_end, float* xt,
-                                 float* x0_pred, int* have_x0, const float* y, const float* noise, int B, void* stream) {
-  DDNM_API_BEGIN
-  DDNM_CHECK(noise, "null argument");
-  sample_simplified_range(static_cast<UNetEngine*>(unet), d, sched, k_begin, k_end, xt, x0_pred, have_x0, y, noise_tape(noise), B,
-                          (cudaStream_t)stream);
-  DDNM_API_END
-}
-int ddnm_sample_simplified_range_seeded(void* unet, const ddnm_simple_deg* d, const ddnm_schedule* sched, int k_begin, int k_end,
-                                        float* xt, float* x0_pred, int* have_x0, const float* y, const ddnm_noise_seed* seed, int B,
-                                        void* stream) {
-  DDNM_API_BEGIN
-  sample_simplified_range(static_cast<UNetEngine*>(unet), d, sched, k_begin, k_end, xt, x0_pred, have_x0, y,
-                          noise_seeded(seed, NZ_LOOP, 0, B), B, (cudaStream_t)stream);
-  DDNM_API_END
-}
-int ddnm_sample_simplified(void* unet, const ddnm_simple_deg* d, const ddnm_schedule* sched, const float* x_T, const float* y,
-                           const float* noise, int B, float* out_x0, float* out_x0_pred, void* stream) {
-  DDNM_API_BEGIN
-  sample_simplified(static_cast<UNetEngine*>(unet), d, sched, x_T, y, noise, B, out_x0, out_x0_pred, (cudaStream_t)stream);
+  simplified_Ap(d, y, B, x, (cudaStream_t)stream);
   DDNM_API_END
 }
 }

@@ -92,6 +92,47 @@ def _noise_mode(noise, seed, row_offset):
     return _lib.noise_seed(seed, row_offset)
 
 
+def _unwrap(model):
+    """The denoiser inside an nn.DataParallel-style wrapper (the model itself when it is not wrapped)."""
+    return model if isinstance(model, _EngineModel) else getattr(model, "module", model)
+
+
+def _schedule(b, eta, sigma_y, plus, config):
+    """The library's ddnm_schedule of the run: the time-travel pairs (svd_ddnm.py:167-206) and the alpha-bar table, kept alive
+    by the returned structure."""
+    pairs = time_pairs(config.diffusion.num_diffusion_timesteps, config.time_travel.T_sampling, config.time_travel.travel_length,
+                       config.time_travel.travel_repeat)
+    abar = np.ascontiguousarray(alpha_bar_table(b).numpy())
+    ti = np.ascontiguousarray(np.array([p[0] for p in pairs], dtype=np.int32))
+    tj = np.ascontiguousarray(np.array([p[1] for p in pairs], dtype=np.int32))
+    s = _lib.Schedule()
+    s.n_pairs, s.t_i, s.t_j, s.abar = len(pairs), ti.ctypes.data, tj.ctypes.data, abar.ctypes.data
+    s.num_timesteps, s.eta, s.sigma_y = int(config.diffusion.num_diffusion_timesteps), float(eta), float(sigma_y)
+    s.plus = 1 if plus else 0
+    s.arrays = (abar, ti, tj)
+    return s
+
+
+def _tape(noise, n_pairs, x):
+    """A caller-supplied tape (tests, seed-for-seed comparisons) on x's device: one draw of x's shape per pair."""
+    if noise is None:
+        return None
+    assert noise.shape == (n_pairs,) + tuple(x.shape)
+    return noise.to(x.device).float().contiguous()
+
+
+def _drive(run, n_pairs, x, noise, ns, rows=None):
+    """The whole schedule through ``run(seeded, k0, k1, src)``, one library call over pairs [k0, k1) with ``src`` its noise argument:
+    seeded noise in one call (the rows a ragged batch was padded with are just further image rows), a caller's tape in one call,
+    otherwise torch-drawn chunks (``_chunked``)."""
+    if ns is not None:
+        run(True, 0, n_pairs, C.byref(ns))
+    elif noise is not None:
+        run(False, 0, n_pairs, _lib.ptr(noise))
+    else:
+        _chunked(n_pairs, x, lambda k0, k1, chunk: run(False, k0, k1, _lib.ptr(chunk)), rows=rows)
+
+
 def _low_res_check(model, low_res, x):
     if isinstance(model, SuperResModel) != (low_res is not None):
         raise ValueError("low_res goes with a SuperResModel denoiser, and only with one")
@@ -102,8 +143,7 @@ def _low_res_check(model, low_res, x):
 def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, noise=None, to_host=True, seed=None, row_offset=0,
          low_res=None):
     ns = _noise_mode(noise, seed, row_offset)
-    if not isinstance(model, _EngineModel):
-        model = getattr(model, "module", model)          # tolerate nn.DataParallel-style wrappers
+    model = _unwrap(model)
     if not isinstance(model, _EngineModel) or not isinstance(A_funcs, _Operator):
         raise TypeError("ddnm_b200.sampler needs a ddnm_b200.model denoiser and a ddnm_b200.operators operator")
     if plus and isinstance(A_funcs, (SRConv, Deblurring2D, CS, GeneralA)):
@@ -115,21 +155,11 @@ def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, n
         if not x.is_cuda:
             x = x.to("cuda", non_blocking=True)            # the reference moves xs[-1] to 'cuda' itself (svd_ddnm.py:45)
         n = x.size(0)
-        pairs = time_pairs(config.diffusion.num_diffusion_timesteps, config.time_travel.T_sampling,
-                           config.time_travel.travel_length, config.time_travel.travel_repeat)
-        abar = np.ascontiguousarray(alpha_bar_table(b).numpy())
-        ti = np.ascontiguousarray(np.array([p[0] for p in pairs], dtype=np.int32))
-        tj = np.ascontiguousarray(np.array([p[1] for p in pairs], dtype=np.int32))
+        s = _schedule(b, eta, sigma_y, plus, config)
         x = x.float().contiguous()
-        if noise is not None:                               # a caller-supplied tape (tests, seed-for-seed comparisons)
-            assert noise.shape == (len(pairs),) + tuple(x.shape)
-            noise = noise.to(x.device).float().contiguous()
+        noise = _tape(noise, s.n_pairs, x)
         yv = y.reshape(n, -1).to(x.device, non_blocking=True).float().contiguous()
         assert yv.shape[1] == A_funcs.y_dim, f"y has {yv.shape[1]} entries per image, operator expects {A_funcs.y_dim}"
-        s = _lib.Schedule()
-        s.n_pairs, s.t_i, s.t_j, s.abar = len(pairs), ti.ctypes.data, tj.ctypes.data, abar.ctypes.data
-        s.num_timesteps, s.eta, s.sigma_y = int(config.diffusion.num_diffusion_timesteps), float(eta), float(sigma_y)
-        s.plus = 1 if plus else 0
         # a ragged last batch rides on an existing bigger engine, padded (classifier guidance keeps the exact size: cls_fn sees n rows)
         eng, eb = (model.engine(n), n) if cls_fn is not None else model.engine_for(n)
         if low_res is not None:
@@ -152,25 +182,14 @@ def _run(x, model, b, eta, A_funcs, y, sigma_y, plus, cls_fn, classes, config, n
         else:
             labels, grad, fn, failure = _guidance(x, model, n, cls_fn)
 
-        def run_range(k0, k1, chunk):
-            rc = _lib.lib().ddnm_sample_range(eng, A_funcs._h, C.byref(s), k0, k1, _lib.ptr(out), _lib.ptr(x0p), C.byref(have_x0),
-                                             _lib.ptr(yv), _lib.ptr(chunk), eb, _lib.ptr(labels), _lib.ptr(grad),
-                                             None if fn is None else C.cast(fn, C.c_void_p), user, _lib.cur_stream())
+        def run(seeded, k0, k1, src):
+            f = _lib.lib().ddnm_sample_range_seeded if seeded else _lib.lib().ddnm_sample_range
+            rc = f(eng, A_funcs._h, C.byref(s), k0, k1, _lib.ptr(out), _lib.ptr(x0p), C.byref(have_x0), _lib.ptr(yv), src, eb,
+                   _lib.ptr(labels), _lib.ptr(grad), None if fn is None else C.cast(fn, C.c_void_p), user, _lib.cur_stream())
             if failure:
                 raise failure[0]
             _lib.check(rc)
-        if ns is not None:
-            # one call over the whole schedule; the rows a ragged batch was padded with are just further image rows
-            rc = _lib.lib().ddnm_sample_range_seeded(eng, A_funcs._h, C.byref(s), 0, len(pairs), _lib.ptr(out), _lib.ptr(x0p),
-                                                    C.byref(have_x0), _lib.ptr(yv), C.byref(ns), eb, _lib.ptr(labels), _lib.ptr(grad),
-                                                    None if fn is None else C.cast(fn, C.c_void_p), user, _lib.cur_stream())
-            if failure:
-                raise failure[0]
-            _lib.check(rc)
-        elif noise is not None:
-            run_range(0, len(pairs), noise)
-        else:
-            _chunked(len(pairs), x, run_range, rows=eb)
+        _drive(run, s.n_pairs, x, noise, ns, rows=eb)
         if eb != n:
             out, x0p = out[:n], x0p[:n]
         if not to_host:
@@ -277,8 +296,7 @@ def simplified_ddnm_plus(x, model, b, eta, degradation, y, sigma_y, config=None,
     ``([x_0.cpu()], [x0_pred.cpu()])`` like the SVD samplers.  ``seed`` / ``row_offset``: library-drawn noise, ``low_res``: the
     conditioning image of a ``SuperResModel``, as in ``ddnm_diffusion``."""
     ns = _noise_mode(noise, seed, row_offset)
-    if not isinstance(model, _EngineModel):
-        model = getattr(model, "module", model)
+    model = _unwrap(model)
     if not isinstance(model, _EngineModel) or not isinstance(degradation, SimplifiedDegradation):
         raise TypeError("simplified_ddnm_plus needs a ddnm_b200.model denoiser and a SimplifiedDegradation")
     _low_res_check(model, low_res, x)
@@ -286,34 +304,19 @@ def simplified_ddnm_plus(x, model, b, eta, degradation, y, sigma_y, config=None,
         if not x.is_cuda:
             x = x.to("cuda", non_blocking=True)
         n = x.size(0)
-        pairs = time_pairs(config.diffusion.num_diffusion_timesteps, config.time_travel.T_sampling,
-                           config.time_travel.travel_length, config.time_travel.travel_repeat)
-        abar = np.ascontiguousarray(alpha_bar_table(b).numpy())
-        ti = np.ascontiguousarray(np.array([p[0] for p in pairs], dtype=np.int32))
-        tj = np.ascontiguousarray(np.array([p[1] for p in pairs], dtype=np.int32))
+        s = _schedule(b, eta, sigma_y, True, config)
         x = x.float().contiguous()
-        if noise is not None:
-            noise = noise.to(x.device).float().contiguous()
+        noise = _tape(noise, s.n_pairs, x)
         yv = y.to(x.device, non_blocking=True).float().contiguous()
-        s = _lib.Schedule()
-        s.n_pairs, s.t_i, s.t_j, s.abar = len(pairs), ti.ctypes.data, tj.ctypes.data, abar.ctypes.data
-        s.num_timesteps, s.eta, s.sigma_y, s.plus = int(config.diffusion.num_diffusion_timesteps), float(eta), float(sigma_y), 1
         out, x0p = x.clone(), torch.empty_like(x)
         eng = model.engine(n)
         if low_res is not None:
             model.stage_low_res(low_res.to(x.device, non_blocking=True), n)
         have_x0 = C.c_int(0)
 
-        def run_range(k0, k1, chunk):
-            _lib.check(_lib.lib().ddnm_sample_simplified_range(eng, C.byref(degradation._d), C.byref(s), k0, k1, _lib.ptr(out),
-                                                              _lib.ptr(x0p), C.byref(have_x0), _lib.ptr(yv), _lib.ptr(chunk), n,
-                                                              _lib.cur_stream()))
-        if ns is not None:
-            _lib.check(_lib.lib().ddnm_sample_simplified_range_seeded(eng, C.byref(degradation._d), C.byref(s), 0, len(pairs),
-                                                                     _lib.ptr(out), _lib.ptr(x0p), C.byref(have_x0), _lib.ptr(yv),
-                                                                     C.byref(ns), n, _lib.cur_stream()))
-        elif noise is not None:
-            run_range(0, len(pairs), noise)
-        else:
-            _chunked(len(pairs), x, run_range)
+        def run(seeded, k0, k1, src):
+            f = _lib.lib().ddnm_sample_simplified_range_seeded if seeded else _lib.lib().ddnm_sample_simplified_range
+            _lib.check(f(eng, C.byref(degradation._d), C.byref(s), k0, k1, _lib.ptr(out), _lib.ptr(x0p), C.byref(have_x0), _lib.ptr(yv),
+                         src, n, _lib.cur_stream()))
+        _drive(run, s.n_pairs, x, noise, ns)
         return [out.to("cpu")], [x0p.to("cpu")]

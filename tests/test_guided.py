@@ -147,3 +147,26 @@ def test_guided_sampler_error_paths(gold):
     # and the engine still works afterwards
     xs, _ = ddnm_diffusion(x_T.cuda(), mu, SCH.linear_betas().cuda(), 0.85, eop, y.cuda(), config=conf, noise=torch.stack(tape).cuda())
     assert torch.isfinite(xs[0]).all()
+
+
+@pytest.mark.gpu
+def test_simplified_ddnm_plus_refuses_a_class_conditional_denoiser():
+    """The simplified loop passes no labels, so a class-conditional denoiser is refused before the first step, as the reference's
+    model(xt, t) asserts for one (unet.py:644-646); a tape shorter than the schedule is refused before the library reads it."""
+    from ddnm_b200._lib import DDNMError
+    from ddnm_b200.sampler import SimplifiedDegradation, simplified_ddnm_plus
+    cfg = _cfg()
+    m = _engine_model(cfg)
+    R = cfg.image_size
+    D = SimplifiedDegradation("colorization", image_size=R)
+    x_T = torch.randn(2, 3, R, R, device="cuda")
+    y = D.A(torch.rand(2, 3, R, R, device="cuda") * 2 - 1)
+    betas = SCH.linear_betas().cuda()
+    conf = sampler_config(4, 1, 1)
+    npairs = len(SCH.time_pairs(1000, 4, 1, 1))
+    with pytest.raises(DDNMError, match="class-conditional"):
+        simplified_ddnm_plus(x_T, m, betas, 0.85, D, y, 0.1, config=conf, noise=torch.randn(npairs, *x_T.shape, device="cuda"))
+    with pytest.raises(DDNMError, match="class-conditional"):
+        simplified_ddnm_plus(x_T, m, betas, 0.85, D, y, 0.1, config=conf, seed=3)
+    with pytest.raises(AssertionError):
+        simplified_ddnm_plus(x_T, m, betas, 0.85, D, y, 0.1, config=conf, noise=torch.randn(npairs - 1, *x_T.shape, device="cuda"))
