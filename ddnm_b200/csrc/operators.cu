@@ -45,7 +45,7 @@ __device__ __forceinline__ void noise_coeff(float s, const PlusScalars& ps, floa
   }
 }
 
-PlusScalars Operator::make_plus(float a, float sigma_y, float sigma_t, float eta) {
+PlusScalars make_plus(float a, float sigma_y, float sigma_t, float eta) {
   PlusScalars p;
   p.a = a; p.sigma_y = sigma_y; p.sigma_t = sigma_t; p.eta = eta;
   p.c = (float)std::sqrt(1.0 - (double)eta * (double)eta);
@@ -537,320 +537,6 @@ __global__ void denoise_kernel(const float* __restrict__ in0, const float* __res
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Operator
-// ------------------------------------------------------------------------------------------------------------------
-template <class T>
-static T* upload(std::vector<void*>& owned, const T* host, size_t n) {
-  T* d = nullptr;
-  CUDA_CHECK(cudaMalloc(&d, std::max<size_t>(n, 1) * sizeof(T)));
-  CUDA_CHECK(cudaMemcpy(d, host, n * sizeof(T), cudaMemcpyHostToDevice));
-  owned.push_back(d);
-  return d;
-}
-static std::vector<float> transpose(const float* m, int r, int c) {
-  std::vector<float> t((size_t)r * c);
-  for (int i = 0; i < r; ++i)
-    for (int j = 0; j < c; ++j) t[(size_t)j * r + i] = m[(size_t)i * c + j];
-  return t;
-}
-
-Operator::Operator(int kind, int channels, int img_dim, int ratio, const float* v_small, const float* u_small,
-                   const float* singulars, const float* singulars_orig, const long long* perm, const long long* mask,
-                   const float* v_small2, const float* u_small2)
-    : kind_(kind), C_(channels), D_(img_dim), ratio_(ratio) {
-  const int n2 = D_ * D_;
-  DDNM_CHECK(channels >= 1 && img_dim >= 2, "bad operator geometry");
-  N_ = (long long)C_ * n2;
-  switch (kind) {
-    case OP_SR: {
-      DDNM_CHECK(ratio >= 1 && img_dim % ratio == 0, "img_dim % ratio");  // svd_operators.py:481
-      // 2 / 4 / 8: one thread per patch with the basis in shared memory; any other ratio (evaluation.sh runs 16x): patch rows +
-      // the K x K basis as a small GEMM
-      sr_generic_ = !(ratio == 2 || ratio == 4 || ratio == 8);
-      DDNM_CHECK(ratio <= 64, "SuperResolution: ratio <= 64");
-      DDNM_CHECK(v_small && u_small && singulars, "SuperResolution needs V_small, U_small, singulars_small");
-      const int K = ratio * ratio;
-      V_ = upload(owned_, v_small, (size_t)K * K);
-      if (sr_generic_) {
-        std::vector<float> v0(K);
-        for (int k = 0; k < K; ++k) v0[k] = v_small[(size_t)k * K];
-        v0_ = upload(owned_, v0.data(), (size_t)K);
-      }
-      u00_ = u_small[0];
-      s0_ = singulars[0];
-      M_ = (long long)C_ * (D_ / ratio) * (D_ / ratio);
-      break;
-    }
-    case OP_COLOR: {
-      DDNM_CHECK(channels == 3 && v_small && u_small && singulars, "Colorization needs 3 channels and its 3x3 basis");
-      V_ = upload(owned_, v_small, 9);
-      u00_ = u_small[0];
-      s0_ = singulars[0];
-      M_ = n2;
-      break;
-    }
-    case OP_INPAINT: {
-      DDNM_CHECK(mask, "Inpainting needs the mask");
-      const long long ne = (long long)n2 * C_;
-      std::vector<int> rank(ne);
-      int r = 0;
-      for (long long e = 0; e < ne; ++e) rank[e] = mask[e] != 0 ? r++ : -1;
-      rank_ = upload(owned_, rank.data(), ne);
-      M_ = r;
-      break;
-    }
-    case OP_WH: {
-      DDNM_CHECK(perm && ratio >= 1, "WalshHadamardCS needs perm");
-      DDNM_CHECK((D_ & (D_ - 1)) == 0 && D_ >= 32 && D_ <= 1024, "WalshHadamardCS: img_dim must be a power of two in [32, 1024]");
-      std::vector<int> p(n2), ip(n2, -1);
-      for (int i = 0; i < n2; ++i) {
-        DDNM_CHECK(perm[i] >= 0 && perm[i] < n2 && ip[perm[i]] < 0, "perm is not a permutation");
-        p[i] = (int)perm[i];
-        ip[perm[i]] = i;
-      }
-      perm_ = upload(owned_, p.data(), n2);
-      invperm_ = upload(owned_, ip.data(), n2);
-      M_ = (long long)C_ * n2 / ratio;
-      break;
-    }
-    case OP_DENOISE:
-      M_ = (long long)C_ * n2;   // svd_operators.py:442-476: A = identity
-      break;
-    case OP_CS: {
-      // ratio field carries cs_size = int(32*32*cs_ratio) (svd_operators.py:111)
-      DDNM_CHECK(v_small && img_dim % 32 == 0 && ratio >= 1 && ratio <= 1024, "CS needs V_small [1024,1024], img_dim % 32, 1 <= cs_size <= 1024");
-      V_ = upload(owned_, v_small, (size_t)1024 * 1024);
-      cs_size_ = ratio;
-      M_ = (long long)C_ * (D_ / 32) * (D_ / 32) * cs_size_;
-      break;
-    }
-    case OP_DEBLUR:
-    case OP_DEBLUR2D: {
-      if (kind == OP_DEBLUR) DDNM_CHECK(singulars_orig != nullptr, "Deblurring needs the un-thresholded singulars");
-      DDNM_CHECK(v_small && u_small && singulars && perm, "Deblurring needs U, V, singular tables and perm");
-      V_ = upload(owned_, v_small, (size_t)n2);
-      U_ = upload(owned_, u_small, (size_t)n2);
-      auto vt = transpose(v_small, D_, D_), ut = transpose(u_small, D_, D_);
-      Vt_ = upload(owned_, vt.data(), (size_t)n2);
-      Ut_ = upload(owned_, ut.data(), (size_t)n2);
-      Vr_ = V_; Vrt_ = Vt_; Ur_ = U_; Urt_ = Ut_;
-      if (kind == OP_DEBLUR2D) {   // svd_operators.py:1094-1166: different 1-D factors on the two sides, no Lambda
-        DDNM_CHECK(v_small2 && u_small2, "Deblurring2D needs the second pair of factors");
-        auto vt2 = transpose(v_small2, D_, D_), ut2 = transpose(u_small2, D_, D_);
-        Vr_ = upload(owned_, v_small2, (size_t)n2);
-        Ur_ = upload(owned_, u_small2, (size_t)n2);
-        Vrt_ = upload(owned_, vt2.data(), (size_t)n2);
-        Urt_ = upload(owned_, ut2.data(), (size_t)n2);
-      }
-      // singulars() = _singulars.repeat(1, 3) is TILED while spectral vectors are (pos, chan)-interleaved
-      // (svd_operators.py:1001 vs :984): D[c][perm[p]] = S[(C*p + c) mod n2]
-      std::vector<float> tD((size_t)C_ * n2), tDi((size_t)C_ * n2), tS(n2);
-      for (int p = 0; p < n2; ++p) {
-        const long long q = perm[p];
-        DDNM_CHECK(q >= 0 && q < n2, "bad perm entry");
-        for (int c = 0; c < C_; ++c) {
-          const float s = singulars[((long long)C_ * p + c) % n2];
-          tD[(size_t)c * n2 + q] = s;
-          tDi[(size_t)c * n2 + q] = s == 0.f ? 0.f : 1.0f / s;
-        }
-        tS[q] = singulars_orig ? singulars_orig[p] : 0.f;
-      }
-      tabD_ = upload(owned_, tD.data(), tD.size());
-      tabDinv_ = upload(owned_, tDi.data(), tDi.size());
-      tabSorig_ = upload(owned_, tS.data(), tS.size());
-      M_ = (long long)C_ * n2;
-      break;
-    }
-    case OP_SRCONV: {
-      DDNM_CHECK(v_small && u_small && singulars && ratio >= 1 && img_dim % ratio == 0, "SRConv needs U_small, V_small, singulars_small");
-      const int sm = D_ / ratio;
-      std::vector<float> vk((size_t)D_ * sm);
-      for (int i = 0; i < D_; ++i)
-        for (int j = 0; j < sm; ++j) vk[(size_t)i * sm + j] = v_small[(size_t)i * D_ + j];
-      auto vkt = transpose(vk.data(), D_, sm);
-      auto ut = transpose(u_small, sm, sm);
-      V_ = upload(owned_, vk.data(), vk.size());     // D x sm
-      Vt_ = upload(owned_, vkt.data(), vkt.size());  // sm x D
-      U_ = upload(owned_, u_small, (size_t)sm * sm);
-      Ut_ = upload(owned_, ut.data(), ut.size());
-      std::vector<float> s2((size_t)sm * sm), s2i((size_t)sm * sm);
-      for (int i = 0; i < sm; ++i)
-        for (int j = 0; j < sm; ++j) {
-          const float s = singulars[i] * singulars[j];
-          s2[(size_t)i * sm + j] = s;
-          s2i[(size_t)i * sm + j] = s == 0.f ? 0.f : 1.0f / s;
-        }
-      tabD_ = upload(owned_, s2.data(), s2.size());
-      tabDinv_ = upload(owned_, s2i.data(), s2i.size());
-      M_ = (long long)C_ * sm * sm;
-      break;
-    }
-    case OP_GENERAL: {
-      // GeneralA (svd_operators.py:173-208): dense A = U diag(s) V^T with FULL factors U [m,m], V [n,n]; only the first m
-      // columns of V ever meet a non-zero coefficient (A(): temp[:, :m]; A_pinv(): add_zeros pads m..n with zeros).
-      // geometry: x is a flat vector of n = img_dim entries per row (channels must be 1)
-      DDNM_CHECK(C_ == 1, "GeneralA: pass channels = 1 and img_dim = n (columns of A)");
-      const long long n = N_ = D_;
-      const int m = ratio;
-      DDNM_CHECK(v_small && u_small && singulars && m >= 1 && m <= n, "GeneralA needs U [m,m], V [n,n], singulars [m] with m <= n");
-      std::vector<float> vm((size_t)n * m), sinv(m);
-      for (long long i = 0; i < n; ++i)
-        for (int j = 0; j < m; ++j) vm[(size_t)i * m + j] = v_small[(size_t)i * n + j];
-      for (int j = 0; j < m; ++j) sinv[j] = singulars[j] == 0.f ? 0.f : 1.0f / singulars[j];   // A_pinv's factors (:74-75)
-      V_ = upload(owned_, vm.data(), vm.size());          // n x m
-      U_ = upload(owned_, u_small, (size_t)m * m);
-      tabD_ = upload(owned_, singulars, (size_t)m);
-      tabDinv_ = upload(owned_, sinv.data(), (size_t)m);
-      M_ = m;
-      break;
-    }
-    default:
-      throw Error("unknown operator kind");
-  }
-}
-
-Operator::~Operator() {
-  for (void* p : owned_) cudaFree(p);
-  for (float* p : scr_)
-    if (p) cudaFree(p);
-}
-
-float* Operator::scratch(int idx, size_t elems) {
-  if (scr_elems_[idx] < elems) {
-    if (scr_[idx]) {
-      CUDA_CHECK(cudaDeviceSynchronize());
-      CUDA_CHECK(cudaFree(scr_[idx]));
-    }
-    CUDA_CHECK(cudaMalloc(&scr_[idx], elems * sizeof(float)));
-    scr_elems_[idx] = elems;
-  }
-  return scr_[idx];
-}
-
-static inline int blocks(long long n, int t = 256) { return (int)cdivll(n, t); }
-
-template <int FN>
-static void local_dispatch(int kind, int ratio, const float* in0, const float* in1, long long in1_stride, const float* in2,
-                           const float* y, const float* V, float u00, float s0, const StepScalars& sc, float* out0, float* out1,
-                           int B, int C, int D, cudaStream_t st, const NoiseSrc& noise = NoiseSrc{}) {   // noise: LF_STEP's draws
-  if (kind == OP_COLOR) {
-    local_launch<3, 1>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, (long long)B * D * D, C, D, st, noise);
-  } else {
-    const long long groups = (long long)B * C * (D / ratio) * (D / ratio);
-    if (ratio == 2) local_launch<4, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, noise);
-    else if (ratio == 4) local_launch<16, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, noise);
-    else local_launch<64, 0>(FN, in0, in1, in1_stride, in2, y, V, u00, s0, sc, out0, out1, groups, C, D, st, noise);
-  }
-}
-
-void Operator::fwht(float* buf, int B, cudaStream_t s) {
-  const long long rows = (long long)B * C_ * D_;
-  const int threads = std::max(128, D_ / 2);
-  const int rpb = threads * 2 / D_;
-  fwht_rows_kernel<<<(int)cdivll(rows, rpb), threads, (size_t)rpb * D_ * 4, s>>>(buf, D_, rows);
-  CUDA_CHECK(cudaGetLastError());
-  const size_t smem = (size_t)D_ * 33 * 4;
-  // the attribute is per device: set it whenever more than the default 48 KiB is needed (a cached process-wide flag would leave
-  // a second GPU of the same process without it)
-  if (smem > 48 * 1024) CUDA_CHECK(cudaFuncSetAttribute(fwht_cols_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  dim3 grid(D_ / 32, B * C_);
-  fwht_cols_kernel<<<grid, 256, smem, s>>>(buf, D_, (float)D_);
-  CUDA_CHECK(cudaGetLastError());
-}
-
-// out[b] = L (lr x lc) * X[b] (lc x rr) * R (rr x rc), X: B*C images; T: scratch of lr*rr per image
-void Operator::sandwich(const float* L, int lr, int lc, const float* X, int B, const float* R, int rr, int rc, float* T,
-                        float* out, cudaStream_t s) {
-  const int nb = B * C_;
-  sgemm_batched(false, nb, 1, lr, rr, lc, 1.0f, L, lc, 0, 0, X, rr, (long long)lc * rr, 0, T, rr, (long long)lr * rr, 0, s);
-  sgemm_batched(false, nb, 1, lr, rc, rr, 1.0f, T, rr, (long long)lr * rr, 0, R, rc, 0, 0, out, rc, (long long)lr * rc, 0, s);
-}
-
-void Operator::deblur_A(const float* x, int B, float* y, cudaStream_t s) {
-  if (kind_ == OP_CS) return cs_A(x, B, y, s);
-  if (kind_ == OP_GENERAL) return general_A(x, B, y, s);
-  const int n2 = D_ * D_;
-  const long long n = (long long)B * C_ * n2;
-  if (kind_ == OP_DEBLUR || kind_ == OP_DEBLUR2D) {
-    float* T = scratch(0, n);
-    float* S = scratch(1, n);
-    sandwich(Vt_, D_, D_, x, B, Vr_, D_, D_, T, S, s);
-    mul_table_kernel<<<blocks(n), 256, 0, s>>>(S, tabD_, 1, C_, n2, n);
-    sandwich(U_, D_, D_, S, B, Urt_, D_, D_, T, y, s);
-  } else {  // SRConv: Vk^T X Vk -> (sm x sm), scale, U . U^T
-    const int sm = D_ / ratio_;
-    float* T = scratch(0, (size_t)B * C_ * sm * D_);
-    float* S = scratch(1, (size_t)B * C_ * sm * sm);
-    float* T2 = scratch(2, (size_t)B * C_ * sm * sm);
-    sandwich(Vt_, sm, D_, x, B, V_, D_, sm, T, S, s);
-    const long long ns = (long long)B * C_ * sm * sm;
-    mul_table_kernel<<<blocks(ns), 256, 0, s>>>(S, tabD_, 0, C_, sm * sm, ns);
-    sandwich(U_, sm, sm, S, B, Ut_, sm, sm, T2, y, s);
-  }
-  CUDA_CHECK(cudaGetLastError());
-}
-
-void Operator::deblur_Apinv(const float* y, int B, float* x, cudaStream_t s) {
-  if (kind_ == OP_CS) return cs_Apinv(y, B, x, s);
-  if (kind_ == OP_GENERAL) return general_Apinv(y, B, x, s);
-  const int n2 = D_ * D_;
-  const long long n = (long long)B * C_ * n2;
-  if (kind_ == OP_DEBLUR || kind_ == OP_DEBLUR2D) {
-    float* T = scratch(0, n);
-    float* S = scratch(1, n);
-    sandwich(Ut_, D_, D_, y, B, Ur_, D_, D_, T, S, s);
-    mul_table_kernel<<<blocks(n), 256, 0, s>>>(S, tabDinv_, 1, C_, n2, n);
-    sandwich(V_, D_, D_, S, B, Vrt_, D_, D_, T, x, s);
-  } else {
-    const int sm = D_ / ratio_;
-    float* S = scratch(1, (size_t)B * C_ * sm * sm);
-    float* T2 = scratch(2, (size_t)B * C_ * sm * sm);
-    float* T = scratch(0, (size_t)B * C_ * sm * D_);
-    sandwich(Ut_, sm, sm, y, B, U_, sm, sm, T2, S, s);
-    const long long ns = (long long)B * C_ * sm * sm;
-    mul_table_kernel<<<blocks(ns), 256, 0, s>>>(S, tabDinv_, 0, C_, sm * sm, ns);
-    // x = Vk (D x sm) * S (sm x sm) * Vk^T (sm x D): first product is D x sm per image
-    const int nb = B * C_;
-    sgemm_batched(false, nb, 1, D_, sm, sm, 1.0f, V_, sm, 0, 0, S, sm, (long long)sm * sm, 0, T, sm, (long long)D_ * sm, 0, s);
-    sgemm_batched(false, nb, 1, D_, D_, sm, 1.0f, T, sm, (long long)D_ * sm, 0, Vt_, D_, 0, 0, x, D_, (long long)D_ * D_, 0, s);
-  }
-  CUDA_CHECK(cudaGetLastError());
-}
-
-// GeneralA: y = U (s * (V^T x)[:m]),  x = V add_zeros((1/s) * (U^T y))  — three small fp32 GEMMs over the batch
-void Operator::general_A(const float* x, int B, float* y, cudaStream_t s) {
-  const int n = (int)x_dim(), m = (int)M_;
-  float* T = scratch(0, (size_t)B * m);
-  sgemm_batched(false, 1, 1, B, m, n, 1.0f, x, n, 0, 0, V_, m, 0, 0, T, m, 0, 0, s);          // T = X Vm
-  mul_table_kernel<<<blocks((long long)B * m), 256, 0, s>>>(T, tabD_, 0, 1, m, (long long)B * m);
-  sgemm_batched(true, 1, 1, B, m, m, 1.0f, T, m, 0, 0, U_, m, 0, 0, y, m, 0, 0, s);           // y[b][k] = sum_j U[k][j] T[b][j]
-}
-void Operator::general_Apinv(const float* y, int B, float* x, cudaStream_t s) {
-  const int n = (int)x_dim(), m = (int)M_;
-  float* T = scratch(0, (size_t)B * m);
-  sgemm_batched(false, 1, 1, B, m, m, 1.0f, y, m, 0, 0, U_, m, 0, 0, T, m, 0, 0, s);          // T[b][j] = sum_k y[b][k] U[k][j]
-  mul_table_kernel<<<blocks((long long)B * m), 256, 0, s>>>(T, tabDinv_, 0, 1, m, (long long)B * m);
-  sgemm_batched(true, 1, 1, B, n, m, 1.0f, T, m, 0, 0, V_, m, 0, 0, x, n, 0, 0, s);           // x[b][i] = sum_j V[i][j] T[b][j]
-}
-
-void Operator::cs_A(const float* x, int B, float* y, cudaStream_t s) {
-  const long long n = (long long)B * C_ * D_ * D_;
-  const int rows = (int)(n / 1024);
-  float* P = scratch(0, n);
-  cs_patch_kernel<true><<<blocks(n), 256, 0, s>>>(x, P, B, C_, D_);
-  // first cs_size coefficients of V^T patch  ==  P [rows x 1024] . V[:, :cs]
-  sgemm_batched(false, 1, 1, rows, cs_size_, 1024, 1.0f, P, 1024, 0, 0, V_, 1024, 0, 0, y, cs_size_, 0, 0, s);
-}
-void Operator::cs_Apinv(const float* y, int B, float* x, cudaStream_t s) {
-  const long long n = (long long)B * C_ * D_ * D_;
-  const int rows = (int)(n / 1024);
-  float* P = scratch(0, n);
-  // V (c, 0, ..)  ==  Y [rows x cs] . V[:, :cs]^T
-  sgemm_batched(true, 1, 1, rows, 1024, cs_size_, 1.0f, y, cs_size_, 0, 0, V_, 1024, 0, 0, P, 1024, 0, 0, s);
-  cs_patch_kernel<false><<<blocks(n), 256, 0, s>>>(P, x, B, C_, D_);
-}
-
-// ------------------------------------------------------------------------------------------------------------------
 // SuperResolution, generic ratio r (K = r*r entries per patch; svd_operators.py:479-623 with r = 16 in evaluation.sh):
 // patches become rows of a [B*C*y*y, K] matrix (row-major inside the patch, the reference's unfold order :510-512).  A has rank 1
 // per patch, so A / A^+ / the projection / Lambda need only V[:, 0] and one dot product per row (V is orthogonal:
@@ -917,323 +603,601 @@ __global__ void srg_rows_kernel(const float* __restrict__ P, const float* __rest
   }
 }
 
-void Operator::srg_A(const float* x, int B, float* y, cudaStream_t s) {
-  const long long n = (long long)B * N_;
-  const int K = ratio_ * ratio_;
-  const long long rows = n / K;
-  float* P = scratch(6, n);
-  sr_patch_kernel<true><<<blocks(n), 256, 0, s>>>(x, P, B, C_, D_, ratio_);
-  srg_rows_kernel<LF_A><<<blocks(rows * 32), 256, 0, s>>>(P, nullptr, nullptr, nullptr, nullptr, v0_, u00_, s0_, PlusScalars{}, y, rows, K);
-}
-void Operator::srg_Apinv(const float* y, int B, float* x, cudaStream_t s) {
-  const long long n = (long long)B * N_;
-  const int K = ratio_ * ratio_;
-  const long long rows = n / K;
-  float* P = scratch(6, n);
-  srg_rows_kernel<LF_PINV><<<blocks(rows * 32), 256, 0, s>>>(nullptr, nullptr, nullptr, nullptr, y, v0_, u00_, s0_, PlusScalars{}, P, rows, K);
-  sr_patch_kernel<false><<<blocks(n), 256, 0, s>>>(P, x, B, C_, D_, ratio_);
-}
-void Operator::srg_project(const float* x0, const float* y, int B, float* out, cudaStream_t s) {
-  const long long n = (long long)B * N_;
-  const int K = ratio_ * ratio_;
-  const long long rows = n / K;
-  float* P = scratch(6, n);
-  float* O = scratch(7, n);
-  sr_patch_kernel<true><<<blocks(n), 256, 0, s>>>(x0, P, B, C_, D_, ratio_);
-  srg_rows_kernel<LF_PROJECT><<<blocks(rows * 32), 256, 0, s>>>(P, nullptr, nullptr, nullptr, y, v0_, u00_, s0_, PlusScalars{}, O, rows, K);
-  sr_patch_kernel<false><<<blocks(n), 256, 0, s>>>(O, out, B, C_, D_, ratio_);
-}
-void Operator::srg_lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s) {
-  const long long n = (long long)B * N_;
-  const int K = ratio_ * ratio_;
-  const long long rows = n / K;
-  float* P = scratch(6, n);
-  float* O = scratch(7, n);
-  sr_patch_kernel<true><<<blocks(n), 256, 0, s>>>(v, P, B, C_, D_, ratio_);
-  srg_rows_kernel<LF_LAMBDA><<<blocks(rows * 32), 256, 0, s>>>(P, nullptr, nullptr, nullptr, nullptr, v0_, u00_, s0_, ps, O, rows, K);
-  sr_patch_kernel<false><<<blocks(n), 256, 0, s>>>(O, out, B, C_, D_, ratio_);
-}
-void Operator::srg_lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s) {
-  const long long n = (long long)B * N_;
-  const int K = ratio_ * ratio_;
-  const long long rows = n / K;
-  float* P = scratch(6, n);
-  float* Q = scratch(7, n);
-  float* Wv = scratch(8, n);
-  float* We = scratch(9, n);
-  sr_patch_kernel<true><<<blocks(n), 256, 0, s>>>(v, P, B, C_, D_, ratio_);
-  sr_patch_kernel<true><<<blocks(n), 256, 0, s>>>(eps, Q, B, C_, D_, ratio_);
-  // W[row][k] = sum_j V[k][j] * raw[row][j]
-  sgemm_batched(true, 1, 1, (int)rows, K, K, 1.0f, P, K, 0, 0, V_, K, 0, 0, Wv, K, 0, 0, s);
-  sgemm_batched(true, 1, 1, (int)rows, K, K, 1.0f, Q, K, 0, 0, V_, K, 0, 0, We, K, 0, 0, s);
-  srg_rows_kernel<LF_NOISE><<<blocks(rows * 32), 256, 0, s>>>(P, Q, Wv, We, nullptr, v0_, u00_, s0_, ps, P, rows, K);
-  sr_patch_kernel<false><<<blocks(n), 256, 0, s>>>(P, out, B, C_, D_, ratio_);
+// ------------------------------------------------------------------------------------------------------------------
+// Operator: the generic paths of the base class, one class per operator family, the factory
+// ------------------------------------------------------------------------------------------------------------------
+Scratch::~Scratch() {
+  if (p_) cudaFree(p_);
 }
 
-void Operator::A(const float* x, int B, float* y, cudaStream_t s) {
-  StepScalars sc{};
-  const int n2 = D_ * D_;
-  if (kind_ == OP_CS) {
-    cs_A(x, B, y, s);
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  if (kind_ == OP_DENOISE) {
-    CUDA_CHECK(cudaMemcpyAsync(y, x, (size_t)B * C_ * n2 * 4, cudaMemcpyDeviceToDevice, s));
-    return;
-  }
-  if (kind_ == OP_SR && sr_generic_) {
-    srg_A(x, B, y, s);
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  switch (kind_) {
-    case OP_SR: case OP_COLOR:
-      local_dispatch<LF_A>(kind_, ratio_, x, nullptr, 0, nullptr, nullptr, V_, u00_, s0_, sc, y, nullptr, B, C_, D_, s);
-      break;
-    case OP_INPAINT:
-      inpaint_kernel<LF_A><<<blocks((long long)B * C_ * n2), 256, 0, s>>>(x, nullptr, 0, nullptr, nullptr, rank_, sc, y, nullptr, B, C_, n2, M_, NoiseSrc{});
-      break;
-    case OP_WH: {
-      const long long n = (long long)B * C_ * n2;
-      float* F = scratch(0, n);
-      CUDA_CHECK(cudaMemcpyAsync(F, x, n * 4, cudaMemcpyDeviceToDevice, s));
-      fwht(F, B, s);
-      wh_spec_kernel<LF_A><<<blocks((long long)B * M_), 256, 0, s>>>(F, nullptr, nullptr, perm_, invperm_, sc.plus, y, B, C_, n2, M_);
-      break;
+float* Scratch::get(size_t elems) {
+  if (elems_ < elems) {
+    if (p_) {
+      CUDA_CHECK(cudaDeviceSynchronize());
+      CUDA_CHECK(cudaFree(p_));
+      p_ = nullptr;
+      elems_ = 0;
     }
-    default: deblur_A(x, B, y, s);
+    CUDA_CHECK(cudaMalloc(&p_, elems * sizeof(float)));
+    elems_ = elems;
   }
-  CUDA_CHECK(cudaGetLastError());
+  return p_;
 }
 
-void Operator::A_pinv(const float* y, int B, float* x, cudaStream_t s) {
-  StepScalars sc{};
-  const int n2 = D_ * D_;
-  if (kind_ == OP_CS) {
-    cs_Apinv(y, B, x, s);
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  if (kind_ == OP_DENOISE) {
-    CUDA_CHECK(cudaMemcpyAsync(x, y, (size_t)B * C_ * n2 * 4, cudaMemcpyDeviceToDevice, s));
-    return;
-  }
-  if (kind_ == OP_SR && sr_generic_) {
-    srg_Apinv(y, B, x, s);
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  switch (kind_) {
-    case OP_SR: case OP_COLOR:
-      local_dispatch<LF_PINV>(kind_, ratio_, nullptr, nullptr, 0, nullptr, y, V_, u00_, s0_, sc, x, nullptr, B, C_, D_, s);
-      break;
-    case OP_INPAINT:
-      inpaint_kernel<LF_PINV><<<blocks((long long)B * C_ * n2), 256, 0, s>>>(nullptr, nullptr, 0, nullptr, y, rank_, sc, x, nullptr, B, C_, n2, M_, NoiseSrc{});
-      break;
-    case OP_WH:
-      wh_spec_kernel<LF_PINV><<<blocks((long long)B * C_ * n2), 256, 0, s>>>(nullptr, nullptr, y, perm_, invperm_, sc.plus, x, B, C_, n2, M_);
-      fwht(x, B, s);
-      break;
-    default: deblur_Apinv(y, B, x, s);
-  }
-  CUDA_CHECK(cudaGetLastError());
+Operator::~Operator() {
+  for (void* p : owned_) cudaFree(p);
+}
+
+template <class T>
+T* Operator::upload(const T* host, size_t n) {
+  T* d = nullptr;
+  CUDA_CHECK(cudaMalloc(&d, std::max<size_t>(n, 1) * sizeof(T)));
+  owned_.push_back(d);
+  CUDA_CHECK(cudaMemcpy(d, host, n * sizeof(T), cudaMemcpyHostToDevice));
+  return d;
+}
+
+static inline int blocks(long long n, int t = 256) { return (int)cdivll(n, t); }
+
+void Operator::residual(const float* x0, const float* y, int B, float* R, cudaStream_t s) {
+  const long long m = (long long)B * M_;
+  float* Ay = ay_.get(m);
+  A(x0, B, Ay, s);
+  sub_kernel<<<blocks(m), 256, 0, s>>>(Ay, y, Ay, m);
+  A_pinv(Ay, B, R, s);
 }
 
 void Operator::project(const float* x0, const float* y, int B, float* out, cudaStream_t s) {
-  StepScalars sc{};
-  const int n2 = D_ * D_;
   const long long n = (long long)B * N_;
-  if (kind_ == OP_DENOISE) {   // x0 - (x0 - y)
-    float* R = scratch(4, n);
-    sub_kernel<<<blocks(n), 256, 0, s>>>(x0, y, R, n);
-    sub_kernel<<<blocks(n), 256, 0, s>>>(x0, R, out, n);
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  if (kind_ == OP_SR && sr_generic_) {
-    srg_project(x0, y, B, out, s);
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  switch (kind_) {
-    case OP_SR: case OP_COLOR:
-      local_dispatch<LF_PROJECT>(kind_, ratio_, x0, nullptr, 0, nullptr, y, V_, u00_, s0_, sc, out, nullptr, B, C_, D_, s);
-      break;
-    case OP_INPAINT:
-      inpaint_kernel<LF_PROJECT><<<blocks(n), 256, 0, s>>>(x0, nullptr, 0, nullptr, y, rank_, sc, out, nullptr, B, C_, n2, M_, NoiseSrc{});
-      break;
-    case OP_WH: {
-      float* F = scratch(0, n);
-      CUDA_CHECK(cudaMemcpyAsync(F, x0, n * 4, cudaMemcpyDeviceToDevice, s));
-      fwht(F, B, s);
-      float* R = scratch(1, n);
-      wh_spec_kernel<LF_PROJECT><<<blocks(n), 256, 0, s>>>(F, nullptr, y, perm_, invperm_, sc.plus, R, B, C_, n2, M_);
-      fwht(R, B, s);
-      sub_kernel<<<blocks(n), 256, 0, s>>>(x0, R, out, n);
-      break;
-    }
-    default: {
-      float* Ay = scratch(3, (size_t)B * M_);
-      float* R = scratch(4, n);
-      deblur_A(x0, B, Ay, s);
-      sub_kernel<<<blocks((long long)B * M_), 256, 0, s>>>(Ay, y, Ay, (long long)B * M_);
-      deblur_Apinv(Ay, B, R, s);
-      sub_kernel<<<blocks(n), 256, 0, s>>>(x0, R, out, n);
-    }
-  }
+  float* R = r_.get(n);
+  residual(x0, y, B, R, s);
+  sub_kernel<<<blocks(n), 256, 0, s>>>(x0, R, out, n);
   CUDA_CHECK(cudaGetLastError());
 }
 
-void Operator::lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s) {
-  StepScalars sc{};
-  sc.plus = ps;
-  const int n2 = D_ * D_;
-  const long long n = (long long)B * C_ * n2;
-  if (kind_ == OP_DENOISE) {
-    denoise_kernel<LF_LAMBDA><<<blocks(n), 256, 0, s>>>(v, nullptr, 0, nullptr, nullptr, sc, out, nullptr, B, (long long)C_ * n2, NoiseSrc{});
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  if (kind_ == OP_DEBLUR2D) throw Error("Deblurring2D defines no Lambda (svd_operators.py:1094-1166): sigma_y > 0 is unsupported, as in the reference");
-  if (kind_ == OP_CS) throw Error("CS defines no Lambda (svd_operators.py:101-159): sigma_y > 0 is unsupported, as in the reference");
-  if (kind_ == OP_GENERAL) throw Error("GeneralA defines no Lambda (svd_operators.py:173-208): sigma_y > 0 is unsupported, as in the reference");
-  if (kind_ == OP_SR && sr_generic_) {
-    srg_lambda(v, B, ps, out, s);
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  switch (kind_) {
-    case OP_SR: case OP_COLOR:
-      local_dispatch<LF_LAMBDA>(kind_, ratio_, v, nullptr, 0, nullptr, nullptr, V_, u00_, s0_, sc, out, nullptr, B, C_, D_, s);
-      break;
-    case OP_INPAINT:
-      inpaint_kernel<LF_LAMBDA><<<blocks(n), 256, 0, s>>>(v, nullptr, 0, nullptr, nullptr, rank_, sc, out, nullptr, B, C_, n2, M_, NoiseSrc{});
-      break;
-    case OP_WH: {
-      float* F = scratch(0, n);
-      CUDA_CHECK(cudaMemcpyAsync(F, v, n * 4, cudaMemcpyDeviceToDevice, s));
-      fwht(F, B, s);
-      wh_spec_kernel<LF_LAMBDA><<<blocks(n), 256, 0, s>>>(F, nullptr, nullptr, perm_, invperm_, ps, out, B, C_, n2, M_);
-      fwht(out, B, s);
-      break;
-    }
-    case OP_DEBLUR: {
-      float* T = scratch(0, n);
-      float* S = scratch(1, n);
-      sandwich(Vt_, D_, D_, v, B, V_, D_, D_, T, S, s);
-      deblur_coeff_kernel<LF_LAMBDA><<<blocks(n), 256, 0, s>>>(S, nullptr, tabSorig_, ps, S, n2, n);
-      sandwich(V_, D_, D_, S, B, Vt_, D_, D_, T, out, s);
-      break;
-    }
-    default:
-      throw Error("SRConv defines no Lambda (svd_operators.py:851-931): sigma_y > 0 is unsupported for sr_bicubic, as in the reference");
-  }
-  CUDA_CHECK(cudaGetLastError());
+void Operator::lambda(const float*, int, const PlusScalars&, float*, cudaStream_t) {
+  throw Error(std::string(name_) + " defines no Lambda (" + src_ + "): sigma_y > 0 is unsupported" + note_ + ", as in the reference");
 }
 
-void Operator::lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s) {
-  StepScalars sc{};
-  sc.plus = ps;
-  const int n2 = D_ * D_;
-  const long long n = (long long)B * C_ * n2;
-  const long long img = (long long)C_ * n2;
-  if (kind_ == OP_DENOISE) {
-    denoise_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, nullptr, 0, nullptr, nullptr, sc, out, nullptr, B, img, NoiseSrc{});
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  if (kind_ == OP_DEBLUR2D) throw Error("Deblurring2D defines no Lambda_noise (svd_operators.py:1094-1166)");
-  if (kind_ == OP_CS) throw Error("CS defines no Lambda_noise (svd_operators.py:101-159)");
-  if (kind_ == OP_GENERAL) throw Error("GeneralA defines no Lambda_noise (svd_operators.py:173-208)");
-  if (kind_ == OP_SR && sr_generic_) {
-    srg_lambda_noise(v, eps, B, ps, out, s);
-    CUDA_CHECK(cudaGetLastError());
-    return;
-  }
-  switch (kind_) {
-    case OP_SR: case OP_COLOR:
-      local_dispatch<LF_NOISE>(kind_, ratio_, v, eps, img, nullptr, nullptr, V_, u00_, s0_, sc, out, nullptr, B, C_, D_, s);
-      break;
-    case OP_INPAINT:
-      inpaint_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, eps, img, nullptr, nullptr, rank_, sc, out, nullptr, B, C_, n2, M_, NoiseSrc{});
-      break;
-    case OP_WH:
-      wh_spec_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, eps, nullptr, perm_, invperm_, ps, out, B, C_, n2, M_);
-      fwht(out, B, s);
-      break;
-    case OP_DEBLUR: {
-      float* T = scratch(0, n);
-      float* S = scratch(1, n);
-      deblur_coeff_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, eps, tabSorig_, ps, S, n2, n);
-      sandwich(V_, D_, D_, S, B, Vt_, D_, D_, T, out, s);
-      break;
-    }
-    default:
-      throw Error("SRConv defines no Lambda_noise (svd_operators.py:851-931)");
-  }
-  CUDA_CHECK(cudaGetLastError());
+void Operator::lambda_noise(const float*, const float*, int, const PlusScalars&, float*, cudaStream_t) {
+  throw Error(std::string(name_) + " defines no Lambda_noise (" + src_ + ")");
 }
 
+// the generic step: x0_t, the residual r = A^+(A x0_t - y), then the DDNM / DDNM+ update
 void Operator::step(const float* xt, const float* et, long long et_stride, const NoiseSrc& nz, const float* y, int B,
                     const StepScalars& sc, float* x0_t, float* xt_next, cudaStream_t s) {
-  const int n2 = D_ * D_;
-  const long long img = N_;
-  const long long n = (long long)B * img;
+  const long long n = (long long)B * N_;
+  float* et3 = et3_.get(n);
+  x0_kernel<<<blocks(n), 256, 0, s>>>(xt, et, et_stride, sc, x0_t, et3, B, N_);
+  float* R = r_.get(n);
+  residual(x0_t, y, B, R, s);
   const float* noise = nz.tape;
-  if ((kind_ == OP_SR && !sr_generic_) || kind_ == OP_COLOR) {
-    local_dispatch<LF_STEP>(kind_, ratio_, xt, et, et_stride, noise, y, V_, u00_, s0_, sc, x0_t, xt_next, B, C_, D_, s, nz);
-  } else if (kind_ == OP_INPAINT) {
+  if (!sc.use_plus) {
     noise_dispatch(nz, [&](auto gen) {
-      inpaint_kernel<LF_STEP, decltype(gen)::value><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, rank_, sc, x0_t, xt_next, B,
-                                                                              C_, n2, M_, nz);
-    });
-  } else if (kind_ == OP_DENOISE) {
-    noise_dispatch(nz, [&](auto gen) {
-      denoise_kernel<LF_STEP, decltype(gen)::value><<<blocks(n), 256, 0, s>>>(xt, et, et_stride, noise, y, sc, x0_t, xt_next, B, img, nz);
+      final_ddnm_kernel<decltype(gen)::value><<<blocks(n), 256, 0, s>>>(x0_t, R, noise, et3, sc, xt_next, n, N_, nz);
     });
   } else {
-    // generic path: x0_t, residual r = A^+(A x0_t - y), then the DDNM / DDNM+ update
-    float* et3 = scratch(5, n);
-    x0_kernel<<<blocks(n), 256, 0, s>>>(xt, et, et_stride, sc, x0_t, et3, B, img);
-    float* R = scratch(4, n);
-    if (kind_ == OP_WH) {
-      float* F = scratch(0, n);
-      CUDA_CHECK(cudaMemcpyAsync(F, x0_t, n * 4, cudaMemcpyDeviceToDevice, s));
-      fwht(F, B, s);
-      wh_spec_kernel<LF_PROJECT><<<blocks(n), 256, 0, s>>>(F, nullptr, y, perm_, invperm_, sc.plus, R, B, C_, n2, M_);
-      fwht(R, B, s);
-    } else {
-      float* Ay = scratch(3, (size_t)B * M_);
-      if (kind_ == OP_SR) {          // generic-ratio SuperResolution
-        srg_A(x0_t, B, Ay, s);
-        sub_kernel<<<blocks((long long)B * M_), 256, 0, s>>>(Ay, y, Ay, (long long)B * M_);
-        srg_Apinv(Ay, B, R, s);
-      } else {
-        deblur_A(x0_t, B, Ay, s);
-        sub_kernel<<<blocks((long long)B * M_), 256, 0, s>>>(Ay, y, Ay, (long long)B * M_);
-        deblur_Apinv(Ay, B, R, s);
-      }
+    if (!noise) {
+      // Lambda_noise of these operators is a transform of the whole draw (a GEMM or a Walsh-Hadamard transform of the raw
+      // pixels), not a map: materialise this ONE pair's draws, the same values the fused kernels make in registers
+      float* Z = z_.get(n);
+      noise_fill(nz, Z, B, N_, s);
+      noise = Z;
     }
-    if (!sc.use_plus) {
-      noise_dispatch(nz, [&](auto gen) {
-        final_ddnm_kernel<decltype(gen)::value><<<blocks(n), 256, 0, s>>>(x0_t, R, noise, et3, sc, xt_next, n, img, nz);
-      });
-    } else {
-      if (!noise) {
-        // Lambda_noise of these operators is a transform of the whole draw (a GEMM or a Walsh-Hadamard transform of the raw
-        // pixels), not a map: materialise this ONE pair's draws, the same values the fused kernels make in registers
-        float* Z = scratch(10, (size_t)n);
-        noise_fill(nz, Z, B, img, s);
-        noise = Z;
-      }
-      lambda(R, B, sc.plus, R, s);                       // R <- Lambda(R)   (in place is safe: inputs are staged first)
-      float* NZ = scratch(3, std::max<size_t>((size_t)n, (size_t)B * M_));
-      lambda_noise(noise, et3, B, sc.plus, NZ, s);
-      final_plus_kernel<<<blocks(n), 256, 0, s>>>(x0_t, R, NZ, sc, xt_next, n);
-    }
+    lambda(R, B, sc.plus, R, s);                       // R <- Lambda(R)   (in place is safe: inputs are staged first)
+    float* NZ = ay_.get(n);
+    lambda_noise(noise, et3, B, sc.plus, NZ, s);
+    final_plus_kernel<<<blocks(n), 256, 0, s>>>(x0_t, R, NZ, sc, xt_next, n);
   }
   CUDA_CHECK(cudaGetLastError());
+}
+
+namespace {
+
+// the step scalars of a fused kernel's Lambda / Lambda_noise form
+StepScalars with_plus(const PlusScalars& ps) {
+  StepScalars sc{};
+  sc.plus = ps;
+  return sc;
+}
+
+std::vector<float> transpose(const float* m, int r, int c) {
+  std::vector<float> t((size_t)r * c);
+  for (int i = 0; i < r; ++i)
+    for (int j = 0; j < c; ++j) t[(size_t)j * r + i] = m[(size_t)i * c + j];
+  return t;
+}
+
+// 1/s, and 0 where s is 0 (A_pinv's factors, svd_operators.py:74-75)
+std::vector<float> reciprocals(const float* s, size_t n) {
+  std::vector<float> r(n);
+  for (size_t i = 0; i < n; ++i) r[i] = s[i] == 0.f ? 0.f : 1.0f / s[i];
+  return r;
+}
+
+// SuperResolution with r = 2, 4, 8 and Colorization: every entry, the step included, is one fused local_kernel launch
+class Local final : public Operator {
+ public:
+  // K: elements of one group (r*r, or 3 for Colorization); V: the K x K basis; u00, s0: U_small[0], singulars[0]
+  Local(int C, int D, int K, const float* V, float u00, float s0)
+      : Operator((long long)C * D * D / K, (long long)C * D * D), C_(C), D_(D), K_(K), V_(upload(V, (size_t)K * K)), u00_(u00),
+        s0_(s0) {}
+  void A(const float* x, int B, float* y, cudaStream_t s) override {
+    launch(LF_A, x, nullptr, 0, nullptr, nullptr, StepScalars{}, y, nullptr, B, s);
+  }
+  void A_pinv(const float* y, int B, float* x, cudaStream_t s) override {
+    launch(LF_PINV, nullptr, nullptr, 0, nullptr, y, StepScalars{}, x, nullptr, B, s);
+  }
+  void project(const float* x0, const float* y, int B, float* out, cudaStream_t s) override {
+    launch(LF_PROJECT, x0, nullptr, 0, nullptr, y, StepScalars{}, out, nullptr, B, s);
+  }
+  void lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    launch(LF_LAMBDA, v, nullptr, 0, nullptr, nullptr, with_plus(ps), out, nullptr, B, s);
+  }
+  void lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    launch(LF_NOISE, v, eps, N_, nullptr, nullptr, with_plus(ps), out, nullptr, B, s);
+  }
+  void step(const float* xt, const float* et, long long et_stride, const NoiseSrc& nz, const float* y, int B, const StepScalars& sc,
+            float* x0_t, float* xt_next, cudaStream_t s) override {
+    launch(LF_STEP, xt, et, et_stride, nz.tape, y, sc, x0_t, xt_next, B, s, nz);
+  }
+
+ private:
+  void launch(int fn, const float* in0, const float* in1, long long in1_stride, const float* in2, const float* y,
+              const StepScalars& sc, float* out0, float* out1, int B, cudaStream_t s, const NoiseSrc& nz = NoiseSrc{}) const {
+    const long long groups = (long long)B * N_ / K_;
+#define LOCAL(K, MODE) local_launch<K, MODE>(fn, in0, in1, in1_stride, in2, y, V_, u00_, s0_, sc, out0, out1, groups, C_, D_, s, nz)
+    switch (K_) {
+      case 3: LOCAL(3, 1); break;
+      case 4: LOCAL(4, 0); break;
+      case 16: LOCAL(16, 0); break;
+      default: LOCAL(64, 0); break;
+    }
+#undef LOCAL
+  }
+  const int C_, D_, K_;
+  const float* V_;
+  const float u00_, s0_;
+};
+
+// SuperResolution with any other ratio: the patch rows of sr_patch_kernel and srg_rows_kernel; the step is the generic one
+class PatchRows final : public Operator {
+ public:
+  // V: the K x K basis; u00, s0: U_small[0], singulars[0]
+  PatchRows(int C, int D, int r, const float* V, float u00, float s0)
+      : Operator((long long)C * (D / r) * (D / r), (long long)C * D * D), C_(C), D_(D), ratio_(r), K_(r * r),
+        V_(upload(V, (size_t)K_ * K_)), u00_(u00), s0_(s0) {
+    std::vector<float> v0(K_);
+    for (int k = 0; k < K_; ++k) v0[k] = V[(size_t)k * K_];
+    v0_ = upload(v0.data(), (size_t)K_);
+  }
+  void A(const float* x, int B, float* y, cudaStream_t s) override {
+    float* P = rows_.get((size_t)B * N_);
+    to_rows(x, P, B, s);
+    row_op<LF_A>(P, nullptr, nullptr, nullptr, nullptr, PlusScalars{}, y, B, s);
+  }
+  void A_pinv(const float* y, int B, float* x, cudaStream_t s) override {
+    float* P = rows_.get((size_t)B * N_);
+    row_op<LF_PINV>(nullptr, nullptr, nullptr, nullptr, y, PlusScalars{}, P, B, s);
+    from_rows(P, x, B, s);
+  }
+  // fused: one pass over the rows (the step's residual still runs through A, sub and A_pinv)
+  void project(const float* x0, const float* y, int B, float* out, cudaStream_t s) override {
+    float* P = rows_.get((size_t)B * N_);
+    float* O = rows2_.get((size_t)B * N_);
+    to_rows(x0, P, B, s);
+    row_op<LF_PROJECT>(P, nullptr, nullptr, nullptr, y, PlusScalars{}, O, B, s);
+    from_rows(O, out, B, s);
+  }
+  void lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    float* P = rows_.get((size_t)B * N_);
+    float* O = rows2_.get((size_t)B * N_);
+    to_rows(v, P, B, s);
+    row_op<LF_LAMBDA>(P, nullptr, nullptr, nullptr, nullptr, ps, O, B, s);
+    from_rows(O, out, B, s);
+  }
+  void lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    const long long n = (long long)B * N_, rows = n / K_;
+    float* P = rows_.get(n);
+    float* Q = rows2_.get(n);
+    float* Wv = wv_.get(n);
+    float* We = we_.get(n);
+    to_rows(v, P, B, s);
+    to_rows(eps, Q, B, s);
+    // W[row][k] = sum_j V[k][j] * raw[row][j]
+    sgemm_batched(true, 1, 1, (int)rows, K_, K_, 1.0f, P, K_, 0, 0, V_, K_, 0, 0, Wv, K_, 0, 0, s);
+    sgemm_batched(true, 1, 1, (int)rows, K_, K_, 1.0f, Q, K_, 0, 0, V_, K_, 0, 0, We, K_, 0, 0, s);
+    row_op<LF_NOISE>(P, Q, Wv, We, nullptr, ps, P, B, s);
+    from_rows(P, out, B, s);
+  }
+
+ private:
+  void to_rows(const float* x, float* P, int B, cudaStream_t s) const {
+    sr_patch_kernel<true><<<blocks((long long)B * N_), 256, 0, s>>>(x, P, B, C_, D_, ratio_);
+  }
+  void from_rows(const float* P, float* x, int B, cudaStream_t s) const {
+    sr_patch_kernel<false><<<blocks((long long)B * N_), 256, 0, s>>>(P, x, B, C_, D_, ratio_);
+    CUDA_CHECK(cudaGetLastError());
+  }
+  template <int FN>
+  void row_op(const float* P, const float* Q, const float* Wv, const float* We, const float* yv, const PlusScalars& ps, float* out,
+              int B, cudaStream_t s) const {
+    const long long rows = (long long)B * N_ / K_;
+    srg_rows_kernel<FN><<<blocks(rows * 32), 256, 0, s>>>(P, Q, Wv, We, yv, v0_, u00_, s0_, ps, out, rows, K_);
+    CUDA_CHECK(cudaGetLastError());
+  }
+  const int C_, D_, ratio_, K_;
+  const float* V_;
+  const float* v0_;   // V[:, 0]
+  const float u00_, s0_;
+  Scratch rows_;      // the input's patch rows (the Lambda_noise output in place)
+  Scratch rows2_;     // the output's patch rows; in Lambda_noise the rows of eps
+  Scratch wv_, we_;   // Lambda_noise: the rows of v and of eps times V^T
+};
+
+// Inpainting: every entry, the step included, is one fused inpaint_kernel launch
+class Inpaint final : public Operator {
+ public:
+  // rank: per (pixel, channel) entry its index in y, or -1 where the mask drops it; M: the kept entries
+  Inpaint(int C, int D, const std::vector<int>& rank, long long M)
+      : Operator(M, (long long)C * D * D), C_(C), HW_(D * D), rank_(upload(rank.data(), rank.size())) {}
+  void A(const float* x, int B, float* y, cudaStream_t s) override {
+    launch<LF_A>(x, nullptr, 0, nullptr, nullptr, StepScalars{}, y, nullptr, B, s);
+  }
+  void A_pinv(const float* y, int B, float* x, cudaStream_t s) override {
+    launch<LF_PINV>(nullptr, nullptr, 0, nullptr, y, StepScalars{}, x, nullptr, B, s);
+  }
+  void project(const float* x0, const float* y, int B, float* out, cudaStream_t s) override {
+    launch<LF_PROJECT>(x0, nullptr, 0, nullptr, y, StepScalars{}, out, nullptr, B, s);
+  }
+  void lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    launch<LF_LAMBDA>(v, nullptr, 0, nullptr, nullptr, with_plus(ps), out, nullptr, B, s);
+  }
+  void lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    launch<LF_NOISE>(v, eps, N_, nullptr, nullptr, with_plus(ps), out, nullptr, B, s);
+  }
+  void step(const float* xt, const float* et, long long et_stride, const NoiseSrc& nz, const float* y, int B, const StepScalars& sc,
+            float* x0_t, float* xt_next, cudaStream_t s) override {
+    noise_dispatch(nz, [&](auto gen) { launch<LF_STEP, decltype(gen)::value>(xt, et, et_stride, nz.tape, y, sc, x0_t, xt_next, B, s, nz); });
+  }
+
+ private:
+  template <int FN, bool GEN = false>
+  void launch(const float* in0, const float* in1, long long in1_stride, const float* in2, const float* y, const StepScalars& sc,
+              float* out0, float* out1, int B, cudaStream_t s, const NoiseSrc& nz = NoiseSrc{}) const {
+    inpaint_kernel<FN, GEN><<<blocks((long long)B * N_), 256, 0, s>>>(in0, in1, in1_stride, in2, y, rank_, sc, out0, out1, B, C_, HW_,
+                                                                       M_, nz);
+    CUDA_CHECK(cudaGetLastError());
+  }
+  const int C_, HW_;
+  const int* rank_;
+};
+
+// Denoising (svd_operators.py:442-476): A = I, so the residual is x0 - y; Lambda, Lambda_noise and the step are fused
+class Denoise final : public Operator {
+ public:
+  explicit Denoise(long long N) : Operator(N, N) {}
+  void A(const float* x, int B, float* y, cudaStream_t s) override {
+    CUDA_CHECK(cudaMemcpyAsync(y, x, (size_t)B * N_ * 4, cudaMemcpyDeviceToDevice, s));
+  }
+  void A_pinv(const float* y, int B, float* x, cudaStream_t s) override {
+    CUDA_CHECK(cudaMemcpyAsync(x, y, (size_t)B * N_ * 4, cudaMemcpyDeviceToDevice, s));
+  }
+  void lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    launch<LF_LAMBDA>(v, nullptr, 0, nullptr, nullptr, with_plus(ps), out, nullptr, B, s);
+  }
+  void lambda_noise(const float* v, const float*, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    launch<LF_NOISE>(v, nullptr, 0, nullptr, nullptr, with_plus(ps), out, nullptr, B, s);
+  }
+  void step(const float* xt, const float* et, long long et_stride, const NoiseSrc& nz, const float* y, int B, const StepScalars& sc,
+            float* x0_t, float* xt_next, cudaStream_t s) override {
+    noise_dispatch(nz, [&](auto gen) { launch<LF_STEP, decltype(gen)::value>(xt, et, et_stride, nz.tape, y, sc, x0_t, xt_next, B, s, nz); });
+  }
+
+ protected:
+  void residual(const float* x0, const float* y, int B, float* R, cudaStream_t s) override {
+    const long long n = (long long)B * N_;
+    sub_kernel<<<blocks(n), 256, 0, s>>>(x0, y, R, n);
+  }
+
+ private:
+  template <int FN, bool GEN = false>
+  void launch(const float* in0, const float* in1, long long in1_stride, const float* in2, const float* y, const StepScalars& sc,
+              float* out0, float* out1, int B, cudaStream_t s, const NoiseSrc& nz = NoiseSrc{}) const {
+    denoise_kernel<FN, GEN><<<blocks((long long)B * N_), 256, 0, s>>>(in0, in1, in1_stride, in2, y, sc, out0, out1, B, N_, nz);
+    CUDA_CHECK(cudaGetLastError());
+  }
+};
+
+// WalshHadamardCS: A keeps M of the transform's coefficients; the residual is one pass in the spectral domain
+class WalshHadamard final : public Operator {
+ public:
+  // perm: the spectral position of each kept coefficient in order; invperm: its inverse
+  WalshHadamard(int C, int D, int ratio, const std::vector<int>& perm, const std::vector<int>& invperm)
+      : Operator((long long)C * D * D / ratio, (long long)C * D * D), C_(C), D_(D), perm_(upload(perm.data(), perm.size())),
+        invperm_(upload(invperm.data(), invperm.size())) {}
+  void A(const float* x, int B, float* y, cudaStream_t s) override {
+    spec<LF_A>(spectrum(x, B, s), nullptr, nullptr, PlusScalars{}, y, B, s);
+  }
+  void A_pinv(const float* y, int B, float* x, cudaStream_t s) override {
+    spec<LF_PINV>(nullptr, nullptr, y, PlusScalars{}, x, B, s);
+    fwht(x, B, s);
+  }
+  void lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    spec<LF_LAMBDA>(spectrum(v, B, s), nullptr, nullptr, ps, out, B, s);
+    fwht(out, B, s);
+  }
+  void lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    spec<LF_NOISE>(v, eps, nullptr, ps, out, B, s);
+    fwht(out, B, s);
+  }
+
+ protected:
+  void residual(const float* x0, const float* y, int B, float* R, cudaStream_t s) override {
+    spec<LF_PROJECT>(spectrum(x0, B, s), nullptr, y, PlusScalars{}, R, B, s);
+    fwht(R, B, s);
+  }
+
+ private:
+  // the transform of x, in scratch
+  float* spectrum(const float* x, int B, cudaStream_t s) {
+    const long long n = (long long)B * N_;
+    float* F = spec_.get(n);
+    CUDA_CHECK(cudaMemcpyAsync(F, x, n * 4, cudaMemcpyDeviceToDevice, s));
+    fwht(F, B, s);
+    return F;
+  }
+  template <int FN>
+  void spec(const float* F, const float* F2, const float* y, const PlusScalars& ps, float* out, int B, cudaStream_t s) const {
+    const long long n = (long long)B * (FN == LF_A ? M_ : N_);
+    wh_spec_kernel<FN><<<blocks(n), 256, 0, s>>>(F, F2, y, perm_, invperm_, ps, out, B, C_, D_ * D_, M_);
+    CUDA_CHECK(cudaGetLastError());
+  }
+  void fwht(float* buf, int B, cudaStream_t s) const {
+    const long long rows = (long long)B * C_ * D_;
+    const int threads = std::max(128, D_ / 2);
+    const int rpb = threads * 2 / D_;
+    fwht_rows_kernel<<<(int)cdivll(rows, rpb), threads, (size_t)rpb * D_ * 4, s>>>(buf, D_, rows);
+    CUDA_CHECK(cudaGetLastError());
+    const size_t smem = (size_t)D_ * 33 * 4;
+    // the attribute is per device: set it whenever more than the default 48 KiB is needed (a cached process-wide flag would leave
+    // a second GPU of the same process without it)
+    if (smem > 48 * 1024) CUDA_CHECK(cudaFuncSetAttribute(fwht_cols_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    dim3 grid(D_ / 32, B * C_);
+    fwht_cols_kernel<<<grid, 256, smem, s>>>(buf, D_, (float)D_);
+    CUDA_CHECK(cudaGetLastError());
+  }
+  const int C_, D_;
+  const int *perm_, *invperm_;
+  Scratch spec_;
+};
+
+// Deblurring, Deblurring2D (svd_operators.py:934-1166) and SRConv (:851-931): per image and channel, the spectrum of X is
+// Vl^T X Vr (k x k), A scales it by the singular table and maps it to y = Ul S Ur^T; A_pinv is the mirror with the reciprocal
+// table.  k = D for the deblurs, the low-resolution side for SRConv.  Only Deblurring defines a Lambda.
+class Separable final : public Operator {
+ public:
+  // vl, vr: D x k; ul, ur: k x k (the same matrices on both sides unless Deblurring2D).  d: the singulars per (channel, spectral
+  // position), or per position when !per_channel.  sorig: Deblurring's un-thresholded singulars per position, empty without a Lambda
+  Separable(int C, int D, int k, const float* vl, const float* vr, const float* ul, const float* ur, const std::vector<float>& d,
+            bool per_channel, const std::vector<float>& sorig, const char* name, const char* src, const char* note = "")
+      : Operator((long long)C * k * k, (long long)C * D * D, name, src, note), C_(C), D_(D), k_(k), per_channel_(per_channel) {
+    vl_ = factor(vl, D, k);
+    vr_ = vr == vl ? vl_ : factor(vr, D, k);
+    ul_ = factor(ul, k, k);
+    ur_ = ur == ul ? ul_ : factor(ur, k, k);
+    d_ = upload(d.data(), d.size());
+    dinv_ = upload(reciprocals(d.data(), d.size()).data(), d.size());
+    if (!sorig.empty()) sorig_ = upload(sorig.data(), sorig.size());
+  }
+  void A(const float* x, int B, float* y, cudaStream_t s) override {
+    float *T = tmp(B), *S = spectral(B);
+    sandwich(vl_.t, k_, D_, x, B, vr_.m, D_, k_, T, S, s);
+    scale(S, d_, B, s);
+    sandwich(ul_.m, k_, k_, S, B, ur_.t, k_, k_, T, y, s);
+  }
+  void A_pinv(const float* y, int B, float* x, cudaStream_t s) override {
+    float *T = tmp(B), *S = spectral(B);
+    sandwich(ul_.t, k_, k_, y, B, ur_.m, k_, k_, T, S, s);
+    scale(S, dinv_, B, s);
+    sandwich(vl_.m, D_, k_, S, B, vr_.t, k_, D_, T, x, s);
+  }
+  void lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    if (!sorig_) return Operator::lambda(v, B, ps, out, s);
+    const long long n = (long long)B * N_;
+    float *T = tmp(B), *S = spectral(B);
+    sandwich(vl_.t, D_, D_, v, B, vl_.m, D_, D_, T, S, s);
+    deblur_coeff_kernel<LF_LAMBDA><<<blocks(n), 256, 0, s>>>(S, nullptr, sorig_, ps, S, D_ * D_, n);
+    sandwich(vl_.m, D_, D_, S, B, vl_.t, D_, D_, T, out, s);
+  }
+  void lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s) override {
+    if (!sorig_) return Operator::lambda_noise(v, eps, B, ps, out, s);
+    const long long n = (long long)B * N_;
+    float *T = tmp(B), *S = spectral(B);
+    deblur_coeff_kernel<LF_NOISE><<<blocks(n), 256, 0, s>>>(v, eps, sorig_, ps, S, D_ * D_, n);
+    sandwich(vl_.m, D_, D_, S, B, vl_.t, D_, D_, T, out, s);
+  }
+
+ private:
+  struct Factor {
+    const float *m, *t;   // the matrix and its transpose
+  };
+  Factor factor(const float* host, int r, int c) {
+    const std::vector<float> t = transpose(host, r, c);
+    return {upload(host, (size_t)r * c), upload(t.data(), t.size())};
+  }
+  // a GEMM's intermediate: at most k x D per image
+  float* tmp(int B) { return t_.get((size_t)B * C_ * k_ * D_); }
+  // the k x k spectrum per image
+  float* spectral(int B) { return s_.get((size_t)B * C_ * k_ * k_); }
+  void scale(float* S, const float* table, int B, cudaStream_t s) const {
+    const long long n = (long long)B * C_ * k_ * k_;
+    mul_table_kernel<<<blocks(n), 256, 0, s>>>(S, table, per_channel_ ? 1 : 0, C_, k_ * k_, n);
+  }
+  // out[b] = L (lr x lc) * X[b] (lc x rr) * R (rr x rc), X: B*C images; T: scratch of lr*rr per image
+  void sandwich(const float* L, int lr, int lc, const float* X, int B, const float* R, int rr, int rc, float* T, float* out,
+                cudaStream_t s) const {
+    const int nb = B * C_;
+    sgemm_batched(false, nb, 1, lr, rr, lc, 1.0f, L, lc, 0, 0, X, rr, (long long)lc * rr, 0, T, rr, (long long)lr * rr, 0, s);
+    sgemm_batched(false, nb, 1, lr, rc, rr, 1.0f, T, rr, (long long)lr * rr, 0, R, rc, 0, 0, out, rc, (long long)lr * rc, 0, s);
+    CUDA_CHECK(cudaGetLastError());
+  }
+  const int C_, D_, k_;
+  const bool per_channel_;
+  Factor vl_, vr_, ul_, ur_;
+  const float *d_, *dinv_, *sorig_ = nullptr;
+  Scratch t_, s_;
+};
+
+// CS (svd_operators.py:101-159): the first cs_size coefficients of each 32 x 32 patch in the basis V
+class Cs final : public Operator {
+ public:
+  // V: the 1024 x 1024 basis
+  Cs(int C, int D, int cs_size, const float* V)
+      : Operator((long long)C * (D / 32) * (D / 32) * cs_size, (long long)C * D * D, "CS", "svd_operators.py:101-159"), C_(C), D_(D),
+        cs_size_(cs_size), V_(upload(V, (size_t)1024 * 1024)) {}
+  void A(const float* x, int B, float* y, cudaStream_t s) override {
+    const long long n = (long long)B * N_;
+    float* P = patches_.get(n);
+    cs_patch_kernel<true><<<blocks(n), 256, 0, s>>>(x, P, B, C_, D_);
+    // first cs_size coefficients of V^T patch  ==  P [rows x 1024] . V[:, :cs]
+    sgemm_batched(false, 1, 1, (int)(n / 1024), cs_size_, 1024, 1.0f, P, 1024, 0, 0, V_, 1024, 0, 0, y, cs_size_, 0, 0, s);
+    CUDA_CHECK(cudaGetLastError());
+  }
+  void A_pinv(const float* y, int B, float* x, cudaStream_t s) override {
+    const long long n = (long long)B * N_;
+    float* P = patches_.get(n);
+    // V (c, 0, ..)  ==  Y [rows x cs] . V[:, :cs]^T
+    sgemm_batched(true, 1, 1, (int)(n / 1024), 1024, cs_size_, 1.0f, y, cs_size_, 0, 0, V_, 1024, 0, 0, P, 1024, 0, 0, s);
+    cs_patch_kernel<false><<<blocks(n), 256, 0, s>>>(P, x, B, C_, D_);
+    CUDA_CHECK(cudaGetLastError());
+  }
+
+ private:
+  const int C_, D_, cs_size_;
+  const float* V_;
+  Scratch patches_;   // the patches as rows of 1024
+};
+
+// GeneralA (svd_operators.py:173-208): y = U (s * (V^T x)[:m]),  x = V add_zeros((1/s) * (U^T y))  — three small fp32 GEMMs
+// over the batch
+class General final : public Operator {
+ public:
+  // Vm: the first m columns of V (n x m), the only ones that meet a non-zero coefficient; U: m x m; sv: the m singulars
+  General(long long n, int m, const std::vector<float>& Vm, const float* U, const float* sv)
+      : Operator(m, n, "GeneralA", "svd_operators.py:173-208"), V_(upload(Vm.data(), Vm.size())), U_(upload(U, (size_t)m * m)),
+        d_(upload(sv, (size_t)m)), dinv_(upload(reciprocals(sv, m).data(), (size_t)m)) {}
+  void A(const float* x, int B, float* y, cudaStream_t s) override {
+    const int n = (int)N_, m = (int)M_;
+    float* T = t_.get((size_t)B * m);
+    sgemm_batched(false, 1, 1, B, m, n, 1.0f, x, n, 0, 0, V_, m, 0, 0, T, m, 0, 0, s);          // T = X Vm
+    mul_table_kernel<<<blocks((long long)B * m), 256, 0, s>>>(T, d_, 0, 1, m, (long long)B * m);
+    sgemm_batched(true, 1, 1, B, m, m, 1.0f, T, m, 0, 0, U_, m, 0, 0, y, m, 0, 0, s);           // y[b][k] = sum_j U[k][j] T[b][j]
+    CUDA_CHECK(cudaGetLastError());
+  }
+  void A_pinv(const float* y, int B, float* x, cudaStream_t s) override {
+    const int n = (int)N_, m = (int)M_;
+    float* T = t_.get((size_t)B * m);
+    sgemm_batched(false, 1, 1, B, m, m, 1.0f, y, m, 0, 0, U_, m, 0, 0, T, m, 0, 0, s);          // T[b][j] = sum_k y[b][k] U[k][j]
+    mul_table_kernel<<<blocks((long long)B * m), 256, 0, s>>>(T, dinv_, 0, 1, m, (long long)B * m);
+    sgemm_batched(true, 1, 1, B, n, m, 1.0f, T, m, 0, 0, V_, m, 0, 0, x, n, 0, 0, s);           // x[b][i] = sum_j V[i][j] T[b][j]
+    CUDA_CHECK(cudaGetLastError());
+  }
+
+ private:
+  const float *V_, *U_, *d_, *dinv_;
+  Scratch t_;   // the m coefficients per row
+};
+
+}  // namespace
+
+Operator* make_operator(const ddnm_operator_desc& d) {
+  const int channels = d.channels, img_dim = d.img_dim, ratio = d.ratio, n2 = img_dim * img_dim;
+  const float *v_small = d.v_small, *u_small = d.u_small, *singulars = d.singulars;
+  const long long* perm = d.perm;
+  DDNM_CHECK(channels >= 1 && img_dim >= 2, "bad operator geometry");
+  switch (d.kind) {
+    case OP_SR: {
+      DDNM_CHECK(ratio >= 1 && img_dim % ratio == 0, "img_dim % ratio");  // svd_operators.py:481
+      DDNM_CHECK(ratio <= 64, "SuperResolution: ratio <= 64");
+      DDNM_CHECK(v_small && u_small && singulars, "SuperResolution needs V_small, U_small, singulars_small");
+      // 2 / 4 / 8: one thread per patch with the basis in shared memory; any other ratio (evaluation.sh runs 16x): patch rows +
+      // the K x K basis as a small GEMM
+      if (ratio == 2 || ratio == 4 || ratio == 8) return new Local(channels, img_dim, ratio * ratio, v_small, u_small[0], singulars[0]);
+      return new PatchRows(channels, img_dim, ratio, v_small, u_small[0], singulars[0]);
+    }
+    case OP_COLOR:
+      DDNM_CHECK(channels == 3 && v_small && u_small && singulars, "Colorization needs 3 channels and its 3x3 basis");
+      return new Local(channels, img_dim, 3, v_small, u_small[0], singulars[0]);
+    case OP_INPAINT: {
+      DDNM_CHECK(d.mask, "Inpainting needs the mask");
+      std::vector<int> rank((size_t)n2 * channels);
+      int r = 0;
+      for (size_t e = 0; e < rank.size(); ++e) rank[e] = d.mask[e] != 0 ? r++ : -1;
+      return new Inpaint(channels, img_dim, rank, r);
+    }
+    case OP_WH: {
+      DDNM_CHECK(perm && ratio >= 1, "WalshHadamardCS needs perm");
+      DDNM_CHECK((img_dim & (img_dim - 1)) == 0 && img_dim >= 32 && img_dim <= 1024,
+                 "WalshHadamardCS: img_dim must be a power of two in [32, 1024]");
+      std::vector<int> p(n2), ip(n2, -1);
+      for (int i = 0; i < n2; ++i) {
+        DDNM_CHECK(perm[i] >= 0 && perm[i] < n2 && ip[perm[i]] < 0, "perm is not a permutation");
+        p[i] = (int)perm[i];
+        ip[perm[i]] = i;
+      }
+      return new WalshHadamard(channels, img_dim, ratio, p, ip);
+    }
+    case OP_DENOISE:
+      return new Denoise((long long)channels * n2);
+    case OP_CS:
+      // ratio carries cs_size = int(32*32*cs_ratio) (svd_operators.py:111)
+      DDNM_CHECK(v_small && img_dim % 32 == 0 && ratio >= 1 && ratio <= 1024, "CS needs V_small [1024,1024], img_dim % 32, 1 <= cs_size <= 1024");
+      return new Cs(channels, img_dim, ratio, v_small);
+    case OP_DEBLUR:
+    case OP_DEBLUR2D: {
+      const bool two = d.kind == OP_DEBLUR2D;   // svd_operators.py:1094-1166: different 1-D factors on the two sides, no Lambda
+      if (!two) DDNM_CHECK(d.singulars_orig != nullptr, "Deblurring needs the un-thresholded singulars");
+      DDNM_CHECK(v_small && u_small && singulars && perm, "Deblurring needs U, V, singular tables and perm");
+      if (two) DDNM_CHECK(d.v_small2 && d.u_small2, "Deblurring2D needs the second pair of factors");
+      // singulars() = _singulars.repeat(1, 3) is TILED while spectral vectors are (pos, chan)-interleaved
+      // (svd_operators.py:1001 vs :984): D[c][perm[p]] = S[(C*p + c) mod n2]
+      std::vector<float> tD((size_t)channels * n2), tS(two ? 0 : n2);
+      for (int p = 0; p < n2; ++p) {
+        const long long q = perm[p];
+        DDNM_CHECK(q >= 0 && q < n2, "bad perm entry");
+        for (int c = 0; c < channels; ++c) tD[(size_t)c * n2 + q] = singulars[((long long)channels * p + c) % n2];
+        if (!two) tS[q] = d.singulars_orig[p];
+      }
+      return new Separable(channels, img_dim, img_dim, v_small, two ? d.v_small2 : v_small, u_small, two ? d.u_small2 : u_small, tD,
+                           true, tS, two ? "Deblurring2D" : "Deblurring", two ? "svd_operators.py:1094-1166" : "svd_operators.py:934-1091");
+    }
+    case OP_SRCONV: {
+      DDNM_CHECK(v_small && u_small && singulars && ratio >= 1 && img_dim % ratio == 0, "SRConv needs U_small, V_small, singulars_small");
+      const int sm = img_dim / ratio;
+      std::vector<float> vk((size_t)img_dim * sm), s2((size_t)sm * sm);   // vk: the first sm columns of V_small
+      for (int i = 0; i < img_dim; ++i)
+        for (int j = 0; j < sm; ++j) vk[(size_t)i * sm + j] = v_small[(size_t)i * img_dim + j];
+      for (int i = 0; i < sm; ++i)
+        for (int j = 0; j < sm; ++j) s2[(size_t)i * sm + j] = singulars[i] * singulars[j];
+      return new Separable(channels, img_dim, sm, vk.data(), vk.data(), u_small, u_small, s2, false, {}, "SRConv", "svd_operators.py:851-931",
+                           " for sr_bicubic");
+    }
+    case OP_GENERAL: {
+      // dense A = U diag(s) V^T with FULL factors U [m,m], V [n,n]; only the first m columns of V ever meet a non-zero coefficient
+      // (A(): temp[:, :m]; A_pinv(): add_zeros pads m..n with zeros).  x is a flat vector of n = img_dim entries per row
+      DDNM_CHECK(channels == 1, "GeneralA: pass channels = 1 and img_dim = n (columns of A)");
+      const long long n = img_dim;
+      const int m = ratio;
+      DDNM_CHECK(v_small && u_small && singulars && m >= 1 && m <= n, "GeneralA needs U [m,m], V [n,n], singulars [m] with m <= n");
+      std::vector<float> vm((size_t)n * m);
+      for (long long i = 0; i < n; ++i)
+        for (int j = 0; j < m; ++j) vm[(size_t)i * m + j] = v_small[(size_t)i * n + j];
+      return new General(n, m, vm, u_small, singulars);
+    }
+    default:
+      throw Error("unknown operator kind");
+  }
 }
 
 }  // namespace ddnm
@@ -1247,8 +1211,7 @@ extern "C" {
 int ddnm_operator_create(const ddnm_operator_desc* d, void** handle) {
   DDNM_API_BEGIN
   DDNM_CHECK(d && handle, "null argument");
-  *handle = new Operator(d->kind, d->channels, d->img_dim, d->ratio, d->v_small, d->u_small, d->singulars, d->singulars_orig,
-                         d->perm, d->mask, d->v_small2, d->u_small2);
+  *handle = make_operator(*d);
   DDNM_API_END
 }
 long long ddnm_operator_y_dim(void* h) { return h ? static_cast<Operator*>(h)->y_dim() : -1; }
@@ -1269,13 +1232,13 @@ int ddnm_operator_project(void* h, const float* x0, const float* y, int B, float
 }
 int ddnm_operator_lambda(void* h, const float* v, int B, float a, float sigma_y, float sigma_t, float eta, float* out, void* stream) {
   DDNM_API_BEGIN
-  static_cast<Operator*>(h)->lambda(v, B, Operator::make_plus(a, sigma_y, sigma_t, eta), out, (cudaStream_t)stream);
+  static_cast<Operator*>(h)->lambda(v, B, make_plus(a, sigma_y, sigma_t, eta), out, (cudaStream_t)stream);
   DDNM_API_END
 }
 int ddnm_operator_lambda_noise(void* h, const float* v, const float* eps, int B, float a, float sigma_y, float sigma_t, float eta,
                                float* out, void* stream) {
   DDNM_API_BEGIN
-  static_cast<Operator*>(h)->lambda_noise(v, eps, B, Operator::make_plus(a, sigma_y, sigma_t, eta), out, (cudaStream_t)stream);
+  static_cast<Operator*>(h)->lambda_noise(v, eps, B, make_plus(a, sigma_y, sigma_t, eta), out, (cudaStream_t)stream);
   DDNM_API_END
 }
 int ddnm_operator_destroy(void* h) {

@@ -3,6 +3,7 @@
 #pragma once
 #include <vector>
 
+#include "../../include/ddnm_b200.h"
 #include "common.cuh"
 #include "noise.cuh"
 
@@ -26,62 +27,69 @@ struct StepScalars {
   int use_plus;
 };
 
+PlusScalars make_plus(float a, float sigma_y, float sigma_t, float eta);
+
+// A device buffer of fp32 that grows on demand.  Growing waits for the device first: work queued earlier may still read the
+// old allocation.
+class Scratch {
+ public:
+  Scratch() = default;
+  Scratch(const Scratch&) = delete;
+  Scratch& operator=(const Scratch&) = delete;
+  ~Scratch();
+  float* get(size_t elems);
+
+ private:
+  float* p_ = nullptr;
+  size_t elems_ = 0;
+};
+
+// One degradation operator (ddnm_operator_create builds it with make_operator).  The defaults are the generic paths: the
+// projection and the step run through A, A_pinv and the Lambdas; operators whose reference class defines no Lambda refuse it.
 class Operator {
  public:
-  Operator(int kind, int channels, int img_dim, int ratio, const float* v_small, const float* u_small, const float* singulars,
-           const float* singulars_orig, const long long* perm, const long long* mask, const float* v_small2 = nullptr,
-           const float* u_small2 = nullptr);
-  ~Operator();
+  virtual ~Operator();
+  Operator(const Operator&) = delete;
+  Operator& operator=(const Operator&) = delete;
   long long y_dim() const { return M_; }
   long long x_dim() const { return N_; }
-  int kind() const { return kind_; }
-  void A(const float* x, int B, float* y, cudaStream_t s);
-  void A_pinv(const float* y, int B, float* x, cudaStream_t s);
-  void project(const float* x0, const float* y, int B, float* out, cudaStream_t s);
-  void lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s);
-  void lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s);
+  virtual void A(const float* x, int B, float* y, cudaStream_t s) = 0;
+  virtual void A_pinv(const float* y, int B, float* x, cudaStream_t s) = 0;
+  // x0 - A^+(A x0 - y)
+  virtual void project(const float* x0, const float* y, int B, float* out, cudaStream_t s);
+  virtual void lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s);
+  virtual void lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s);
   // One sampler step: x0_t = (xt - et*sqrt(1-at))/sqrt(at); x0_hat by projection (and Lambda); xt_next.
   // et_stride = elements between consecutive images of et (6-channel nets keep channels 0..2).
   // noise: a tape of this pair's draws, or a generated source (noise.cuh): the fused kernels then produce the values in
   // registers, and the operators whose Lambda_noise is a transform fill one pair's worth of scratch first.
-  void step(const float* xt, const float* et, long long et_stride, const NoiseSrc& noise, const float* y, int B, const StepScalars& sc,
-            float* x0_t, float* xt_next, cudaStream_t s);
-  static PlusScalars make_plus(float a, float sigma_y, float sigma_t, float eta);
+  virtual void step(const float* xt, const float* et, long long et_stride, const NoiseSrc& noise, const float* y, int B,
+                    const StepScalars& sc, float* x0_t, float* xt_next, cudaStream_t s);
+
+ protected:
+  // M, N: per-image lengths of y and x.  name, src, note: the reference class and its source lines, and what the refusal of an
+  // undefined Lambda adds to "sigma_y > 0 is unsupported"
+  Operator(long long M, long long N, const char* name = "", const char* src = "", const char* note = "")
+      : M_(M), N_(N), name_(name), src_(src), note_(note) {}
+  // R = A^+(A x0 - y)
+  virtual void residual(const float* x0, const float* y, int B, float* R, cudaStream_t s);
+  // a device copy of n host elements, freed with the operator
+  template <class T>
+  T* upload(const T* host, size_t n);
+
+  const long long M_, N_;
 
  private:
-  float* scratch(int idx, size_t elems);
-  void fwht(float* buf, int B, cudaStream_t s);
-  void sandwich(const float* L, int lr, int lc, const float* X, int B, const float* R, int rr, int rc, float* T, float* out,
-                cudaStream_t s);
-  void deblur_A(const float* x, int B, float* y, cudaStream_t s);
-  void deblur_Apinv(const float* y, int B, float* x, cudaStream_t s);
-
-  void general_A(const float* x, int B, float* y, cudaStream_t s);
-  void general_Apinv(const float* y, int B, float* x, cudaStream_t s);
-  // SuperResolution with a ratio other than 2 / 4 / 8 (e.g. the paper's 16x): patch rows + the K x K basis as a small GEMM
-  bool sr_generic_ = false;
-  float* v0_ = nullptr;   // V_small[:, 0]
-  void srg_A(const float* x, int B, float* y, cudaStream_t s);
-  void srg_Apinv(const float* y, int B, float* x, cudaStream_t s);
-  void srg_project(const float* x0, const float* y, int B, float* out, cudaStream_t s);
-  void srg_lambda(const float* v, int B, const PlusScalars& ps, float* out, cudaStream_t s);
-  void srg_lambda_noise(const float* v, const float* eps, int B, const PlusScalars& ps, float* out, cudaStream_t s);
-  void cs_A(const float* x, int B, float* y, cudaStream_t s);
-  void cs_Apinv(const float* y, int B, float* x, cudaStream_t s);
-  int cs_size_ = 0;
-  int kind_, C_, D_, ratio_;
-  long long M_ = 0, N_ = 0;   // per-image lengths of y and x
-  // device artefacts
-  float *V_ = nullptr, *Vt_ = nullptr, *U_ = nullptr, *Ut_ = nullptr;
-  float *Vr_ = nullptr, *Vrt_ = nullptr, *Ur_ = nullptr, *Urt_ = nullptr;   // right-hand factors (== left ones unless Deblurring2D)
-  float u00_ = 1.f, s0_ = 1.f;
-  float *tabD_ = nullptr, *tabDinv_ = nullptr, *tabSorig_ = nullptr;  // deblur: per (c, pos) / per pos tables; srconv: S2, S2inv
-  int *rank_ = nullptr;      // inpaint: kept-rank per pixel or -1
-  int *perm_ = nullptr, *invperm_ = nullptr;
+  const char *name_, *src_, *note_;
   std::vector<void*> owned_;
-  float* scr_[11] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  size_t scr_elems_[11] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};   // [10]: one pair of generated draws (step, seeded DDNM+)
+  Scratch ay_;    // A x0 - y in residual(); the step's Lambda_noise output once that is consumed
+  Scratch r_;     // the residual of project() and step()
+  Scratch et3_;   // step: the epsilon channels the update uses
+  Scratch z_;     // step: one pair of generated draws (seeded DDNM+)
 };
+
+// validates the descriptor and builds the operator of its kind; throws Error with the reason otherwise
+Operator* make_operator(const ddnm_operator_desc& d);
 
 // simplified.cu: the runner's image-space degradations (mask / colour-to-gray / average-pool, diffusion.py:244-290) on
 // (B, 3, D, D) images

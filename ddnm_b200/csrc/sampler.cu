@@ -124,7 +124,7 @@ struct SvdStep {
   void operator()(const float* xt, const float* et, long long et_stride, const NoiseSrc& z, StepScalars s, float at_next, float* x0t,
                   float* xn) const {
     s.use_plus = sc->plus ? 1 : 0;
-    if (s.use_plus) s.plus = Operator::make_plus(s.sqrt_atn, sc->sigma_y, std::sqrt(1.0f - at_next), sc->eta);
+    if (s.use_plus) s.plus = make_plus(s.sqrt_atn, sc->sigma_y, std::sqrt(1.0f - at_next), sc->eta);
     op->step(xt, et, et_stride, z, y, B, s, x0t, xn, st);
   }
 };

@@ -448,7 +448,8 @@ def test_sampler_single_steps_teacher_forced(gold):
     sd = U.init_state_dict(cfg, 1234)
     m = _engine_model(cfg)
     betas_c = torch.from_numpy(g["betas"])
-    for name, sy in (("sr4", 0.0), ("sr4", 0.1), ("color", 0.1), ("inpaint", 0.1), ("wh", 0.1), ("deblur", 0.1), ("bicubic", 0.0)):
+    for name, sy in (("sr4", 0.0), ("sr4", 0.1), ("color", 0.1), ("inpaint", 0.1), ("wh", 0.1), ("deblur", 0.1), ("bicubic", 0.0),
+                     ("denoise", 0.1), ("deblur2d", 0.0), ("cs", 0.0)):
         oop = oracle_ops(gold["operators"], 32)[name]
         eop = engine_op(name, oop, 32)
         torch.manual_seed(21)
